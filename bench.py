@@ -1,6 +1,6 @@
-"""bench.py -- agent-env-steps/sec of the CACC + A2C + NeurComm hot path on B200.
+"""bench.py -- agent-env-steps/sec of the CACC + A2C + NeurComm hot path on H100.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
 A "step" is one full update of the hot path over one batch: n_step (60) env steps of B parallel
@@ -20,6 +20,10 @@ backward cell kernel and the weight-gradient GEMM.  `cpu_baseline` times the res
 unavailable) on the host cores.  `configs` holds the other BASELINE.json configurations at their TOTAL env
 counts split over the N ranks (cfg2 strong-scaling point, cfg3 CommNet, cfg4 DIAL, cfg5 5x5 grid), and
 `dropin_b1` the reference-facing list/NumPy API at one env (main.py train's loop).
+
+--dump-outputs DIR writes, after the timed steps, what the last timed update handed its caller (updated parameters,
+gradient norms, loss terms, per-step global rewards) as DIR/<name>.npy, so two builds can be compared output for
+output: the inputs depend only on the fixed seeds and the arguments.
 """
 import argparse
 import json
@@ -47,6 +51,7 @@ def parse():
     ap.add_argument('--no-cpu-baseline', action='store_true')
     ap.add_argument('--no-e2e', action='store_true')
     ap.add_argument('--no-extra', action='store_true', help='skip the `configs` block and the B=1 drop-in timing')
+    ap.add_argument('--dump-outputs', metavar='DIR', help='write the outputs of the last timed update as DIR/<name>.npy')
     return ap.parse_args()
 
 
@@ -110,7 +115,7 @@ def cpu_reference(cfg_name, updates, warm_updates=1):
 
 
 class ClockSampler:
-    """Streams `nvidia-smi -lms 100` while the timed region runs (B200_PROFILING.md clocks line)."""
+    """Streams `nvidia-smi -lms 100` while the timed region runs (SM clock and throttle reasons beside the number)."""
     Q = 'clocks.sm,clocks.max.sm,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,' \
         'clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap'
 
@@ -238,7 +243,7 @@ class Runner:
             dist.all_reduce(ms, op=dist.ReduceOp.MAX)
         return float(ms.item())
 
-    def measure(self, env, model, steps, warmup, e2e=True, clocks=False):
+    def measure(self, env, model, steps, warmup, e2e=True, clocks=False, dump=None):
         import torch
         from deeprl_network_b200.utils import VecTrainer
         e = model.engine
@@ -247,8 +252,8 @@ class Runner:
         out = {'envs_per_gpu': B, 'global_envs': B * self.world, 'agents': N, 'n_step': T,
                'tensor_core_path': bool(e.use_tc)}
         if not e.use_tc:
-            out['note'] = 'FP32 FFMA fallback kernels (needs envs_per_gpu % 128 == 0 and narrow encoders for tcgen05)'
-            sys.stderr.write('[bench] WARNING: %s x %d envs runs on the FFMA fallback kernels, not tcgen05\n' % (env.agent, B))
+            out['note'] = 'FP32 FFMA fallback kernels (needs envs_per_gpu % 128 == 0 and narrow encoders for the tensor cores)'
+            sys.stderr.write('[bench] WARNING: %s x %d envs runs on the FFMA fallback kernels, not the tensor cores\n' % (env.agent, B))
         vt = VecTrainer(env, model, graph=True, sample='philox')
         vt.start()
         l0 = e.launches
@@ -263,6 +268,8 @@ class Runner:
         ms = self.timed(vt.update, steps)
         if sampler is not None:
             out['clocks'] = sampler.summary()
+        if dump is not None:
+            dump_outputs(dump, e)
         out['value'] = steps * per_update * self.world / (ms * 1e-3)
         out['ms_per_step'] = ms / steps
         if e2e:
@@ -309,6 +316,16 @@ class Runner:
         return out
 
 
+def dump_outputs(dirname, e):
+    """The results of the engine's last update as float32 / float64 .npy files (a few MB at the default sizes)."""
+    import numpy as np
+    os.makedirs(dirname, exist_ok=True)
+    outs = {'params': e.params, 'grad_norm': e.norm_out, 'loss_terms': e.loss_part.sum(dim=(0, 2)), 'global_rewards': e.grew_buf}
+    for name, t in outs.items():
+        a = t.detach().cpu().numpy()
+        np.save(os.path.join(dirname, name + '.npy'), a.astype(np.float64 if a.dtype == np.float64 else np.float32))
+
+
 def kernel_rooflines(env, model, vt, peaks, runner):
     """In-situ CUDA-event durations of the three tensor-core kernels of one eagerly launched update, and the
     SURVEY-8(d) roofline numbers built from them."""
@@ -318,9 +335,9 @@ def kernel_rooflines(env, model, vt, peaks, runner):
     e = model.engine
     T, N, B = e.T, e.N, e.B
     lay = model.layout
-    peak = float(peaks.get('hbm_gbs', 6650.0))
-    tf32_peak = float(peaks.get('bf16_tflops', 1590.0)) / 2
-    src = 'MEASURED_PEAKS.json (burst)' if peaks else 'fallback 6.65 TB/s / 1.59 PF bf16'
+    peak = float(peaks.get('hbm_gbs', 3350.0))
+    tf32_peak = float(peaks.get('bf16_tflops', 989.0)) / 2
+    src = 'MEASURED_PEAKS.json (burst)' if peaks else 'H100 SXM data sheet 3.35 TB/s / 989 TF bf16 dense (not measured)'
     b_step = survey_bytes(env.agent, 5, e.n_a, env.neighbor_mask, env.coop_gamma < 0)
     traffic = {}
     try:
@@ -376,7 +393,7 @@ def kernel_rooflines(env, model, vt, peaks, runner):
                 'traffic': ncu_b, 'dram_frac': None if ncu_b is None else ncu_b / (us * 1e-6) / 1e9 / peak,
                 'issued_tf32_tflops': flops / (us * 1e-6) / 1e12, 'tensor_frac': flops / (us * 1e-6) / 1e12 / tf32_peak}
     fwd = triple(b_step * N * B, fwd_us, t_fwd, f_fwd)
-    r = {'kernel': 'tc_cell_fwd_kernel<PS> (tcgen05 3xTF32: fused gather + encoders + LSTM cell + heads + sampling + '
+    r = {'kernel': 'tc_cell_fwd_kernel<PS> (wgmma 3xTF32: fused gather + encoders + LSTM cell + heads + sampling + '
                    'activation save; rollout p-call)', 'bound': 'hbm', 'unit': 'GB/s', 'peak': peak, 'peak_source': src,
          'tf32_peak_tflops': tf32_peak,
          'timing': 'CUDA events on the launching stream around each launch of one eagerly launched update (in situ)',
@@ -457,7 +474,8 @@ def main():
     cp, env, model = build(args.config, B, rank)
     e = model.engine
     T, N = e.T, e.N
-    head = runner.measure(env, model, args.steps, args.warmup, e2e=not args.no_e2e, clocks=True)
+    head = runner.measure(env, model, args.steps, args.warmup, e2e=not args.no_e2e, clocks=True,
+                          dump=args.dump_outputs if rank == 0 else None)
     peaks = {}
     try:
         peaks = json.load(open(os.path.join(ROOT, 'MEASURED_PEAKS.json')))

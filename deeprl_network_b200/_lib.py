@@ -137,4 +137,4 @@ def stream():
 
 def require_cuda():
     if not torch.cuda.is_available():
-        raise RuntimeError('deeprl_network_b200 needs a CUDA device (sm_100a); no CPU fallback exists')
+        raise RuntimeError('deeprl_network_b200 needs a CUDA device (sm_90a); no CPU fallback exists')

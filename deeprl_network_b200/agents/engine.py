@@ -45,7 +45,7 @@ class PolicyEngine:
         self.grads = torch.zeros(layout.n_param, **f32)
         self.ms = torch.ones(layout.n_param, **f32)             # TF RMSProp slot starts at 1
         self.wt = torch.zeros(layout.n_wt, **f32)
-        # tcgen05 path: packed 3xTF32 operands; used by the kernels when B % 128 == 0
+        # tensor-core path: packed 3xTF32 operands; used by the kernels when B % 128 == 0
         if use_tc is None:
             use_tc = os.environ.get('NMARL_NO_TC', '0') != '1'
         # same conditions as nmarl_tc_fwd_supported / the bptt dispatch (csrc): whole 128-env tiles, narrow encoders
@@ -137,7 +137,7 @@ class PolicyEngine:
         """Host sync: raise if the tensor-core pipeline watchdog fired."""
         code = int(self.tc_err.item())
         if code:
-            raise RuntimeError('tcgen05 pipeline watchdog fired (code %d)' % code)
+            raise RuntimeError('tensor-core pipeline watchdog fired (code %d)' % code)
 
     def _refresh_msg(self):
         if self.variant == 'ma2c_dial':
@@ -340,7 +340,7 @@ class PolicyEngine:
         self.sv_enc = z(T, N, B, 128) if self.variant in ('ma2c_ic3', 'ma2c_dial') else None
         self.sv_dlv = z(T, N, B, 8)
         # tensor-core path: sv_dz holds per-tile gate-bias partial sums, sv_dpre is unused (operand tiles instead)
-        self.sv_dz = z(T, N, B // 128, 4 * NH) if self.use_tc else z(T, N, B, 4 * NH)
+        self.sv_dz = z(T, N, B // 32, 4 * NH) if self.use_tc else z(T, N, B, 4 * NH)
         self.sv_dpre = z(4) if self.use_tc else z(T, N, B, 192)
         # tensor-core path: dz / encoder pre-activation gradients additionally as K-major [hi | lo] operand tiles
         ndp = {'ma2c_nc': 192, 'ia2c': 64}.get(self.variant, 128)

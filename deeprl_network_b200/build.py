@@ -1,4 +1,4 @@
-"""Build libnmarl.so in-tree with nvcc for sm_100a (cross-compiles without a GPU).
+"""Build libnmarl.so in-tree with nvcc for sm_90a (cross-compiles without a GPU).
 
     python -m deeprl_network_b200.build [--force]
 
@@ -14,7 +14,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, 'csrc')
 LIB = os.path.join(HERE, 'libnmarl.so')
 SOURCES = [('api.cu', []), ('env.cu', ['--fmad=false']), ('cell_fwd.cu', []), ('train.cu', []), ('tc_gemm.cu', []), ('tc_cell.cu', []), ('tc_bwd.cu', []), ('tc_wgrad.cu', [])]
-ARCH = ['-gencode', 'arch=compute_100a,code=sm_100a']
+ARCH = ['-gencode', 'arch=compute_90a,code=sm_90a']
 COMMON = ['-O3', '-lineinfo', '-std=c++17', '-Xcompiler', '-fPIC', '-Xcompiler', '-fvisibility=hidden']
 
 

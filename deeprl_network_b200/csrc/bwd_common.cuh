@@ -1,5 +1,5 @@
 // bwd_common.cuh -- argument block of one reverse step, shared by cell_bwd_kernel (FFMA, train.cu) and
-// tc_cell_bwd_kernel (tcgen05, tc_bwd.cu)
+// tc_cell_bwd_kernel (tensor cores, tc_bwd.cu)
 #pragma once
 #include "common.cuh"
 
@@ -18,8 +18,8 @@ struct BwdK {
   const float* c_prev; const float* c_cur;      // c_seq[t], c_seq[t+1]
   const float* dh_in; const float* dc_in; const float* dmsg_in;       // produced by step t+1
   float* dh_out; float* dc_out; float* dmsg_out;                       // consumed by step t-1
-  float* sv_dz; float* sv_dpre;                                        // step t (tcgen05 path: sv_dz = [N][tiles][256] gate-bias partials)
-  const float* wpack; int* tc_err;                                     // tcgen05 path (NULL -> FFMA)
+  float* sv_dz; float* sv_dpre;                                        // step t (tensor-core path: sv_dz = [N][B/32][256] gate-bias partials)
+  const float* wpack; int* tc_err;                                     // tensor-core path (NULL -> FFMA)
   float* dzT;                                                          // step t: [N][B/32][hi|lo][256][32] tiles or NULL
   float* dpT;                                                          // step t: [N][B/32][hi|lo][ndp][32] tiles (encoder pre-act grads)
   int state_fm;                                                        // c/dh/dc/dmsg tensors are feature-major

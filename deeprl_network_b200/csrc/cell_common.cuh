@@ -1,4 +1,4 @@
-// cell_common.cuh -- argument block shared by the FFMA (cell_fwd.cu) and tcgen05 (tc_cell.cu) forward kernels
+// cell_common.cuh -- argument block shared by the FFMA (cell_fwd.cu) and tensor-core (tc_cell.cu) forward kernels
 #pragma once
 #include "common.cuh"
 
@@ -16,6 +16,6 @@ struct FwdK {
 };
 extern long long* g_nmarl_prof;          // set by nmarl_debug_set_prof
 
-// tcgen05 path (tc_cell.cu): returns 0 on success
+// tensor-core path (tc_cell.cu): returns 0 on success
 int nmarl_tc_launch_fwd(const nmarl_model* m, const FwdK& k, int mode, cudaStream_t st);
 bool nmarl_tc_fwd_supported(const nmarl_model* m, const nmarl_fwd_args* a);

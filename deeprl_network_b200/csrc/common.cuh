@@ -1,4 +1,4 @@
-// common.cuh -- shared device helpers for libnmarl (sm_100a only).
+// common.cuh -- shared device helpers for libnmarl (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

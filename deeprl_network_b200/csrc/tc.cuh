@@ -1,15 +1,14 @@
-// tc.cuh -- Blackwell (sm_100a) tensor-core primitives used by the 3xTF32 GEMMs:
-// tcgen05.mma kind::tf32 with the A operand in TMEM, the B operand in 128B-swizzled shared memory
-// (staged by cp.async.bulk + mbarrier), FP32 accumulators in TMEM, tcgen05.ld/st for the
-// register <-> TMEM traffic.  Inline PTX only (no CUTLASS dependency).
+// tc.cuh -- Hopper (sm_90a) tensor-core primitives used by the 3xTF32 GEMMs:
+// wgmma.mma_async kind tf32 with both operands in 128B-swizzled shared memory (the weight operand staged by
+// cp.async.bulk + mbarrier, the activation operand written by the CUDA cores), FP32 accumulators in the registers of
+// the issuing warpgroup.  Inline PTX only (no CUTLASS dependency).
 //
 // fp32-accurate products on TF32 tensor cores ("3xTF32"): x = hi + lo with hi = x ROUNDED to TF32
 // (cvt.rna.tf32) and lo = the remainder x - hi (exact in fp32) rounded to TF32 as well.
 // a*b ~= a_hi*b_hi + a_hi*b_lo + a_lo*b_hi; the dropped terms are O(2^-22 |a||b|) and -- because both parts are
 // rounded to nearest -- zero-mean.  (The cheaper split, hi = x & 0xFFFFE000 with the hardware truncating lo, makes
 // hi, lo and the dropped lo*lo term all err toward zero: a systematic ~2e-7 relative bias per product that does not
-// average out over long contractions and is amplified by cancellation -- measured 3.6e-5 of max|g| on the 245 760-row
-// weight gradients at B = 4096, T = 60, 60x the error of plain fp32 arithmetic.)  Accumulation is FP32 in TMEM.
+// average out over long contractions and is amplified by cancellation.)  Accumulation is FP32.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -47,9 +46,8 @@ __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)_
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 
-// One elected lane of a converged warp.  ptxas treats a branch on elect.sync as single-threaded, so the operands of the
-// tcgen05.mma / commit instructions inside it move to uniform registers with a plain R2UR instead of the per-operand
-// ELECT + R2UR.BROADCAST + BRA.U.ANY waterfall loop it emits under `if (lane == 0)` (~100 cycles per MMA).
+// One elected lane of a converged warp (the bulk-copy producer).  ptxas treats a branch on elect.sync as
+// single-threaded, so the copy operands stay in uniform registers.
 __device__ __forceinline__ bool elect_one() {
   uint32_t pred;
   asm volatile(
@@ -107,114 +105,84 @@ __device__ __forceinline__ void bulk_g2s(void* smem_dst, const void* gsrc, uint3
                : "memory");
 }
 
-// ---- TMEM -------------------------------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_dst, uint32_t ncols) {   // one full warp
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)), "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {     // same warp that allocated
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void fence_before_sync() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void fence_after_sync() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-
-// 32 lanes x 32 bit, 16 consecutive columns: thread i of the warp <-> TMEM lane (warp%4)*32 + i
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, float (&v)[16]) {
-  uint32_t r[16];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-#pragma unroll
-  for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
-}
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16};" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]),
-      "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-      : "memory");
-}
-
-__device__ __forceinline__ void tmem_st8(uint32_t taddr, const uint32_t (&r)[8]) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"r"(taddr), "r"(r[0]), "r"(r[1]),
-               "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7])
-               : "memory");
-}
-__device__ __forceinline__ void tmem_ld8(uint32_t taddr, float (&v)[8]) {
-  uint32_t r[8];
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-               : "r"(taddr)
-               : "memory");
-#pragma unroll
-  for (int i = 0; i < 8; ++i) v[i] = __uint_as_float(r[i]);
-}
-__device__ __forceinline__ void tmem_st_hilo8(uint32_t taddr_hi, uint32_t taddr_lo, const float (&x)[8]) {
-  uint32_t hi[8], lo[8];
-#pragma unroll
-  for (int i = 0; i < 8; ++i) {
-    split_tf32(x[i], hi[i], lo[i]);
-  }
-  tmem_st8(taddr_hi, hi);
-  tmem_st8(taddr_lo, lo);
-}
-
-// hi/lo split of 16 fp32 values and store as two TF32 operand chunks (hi at col, lo at col + lo_off)
-__device__ __forceinline__ void tmem_st_hilo16(uint32_t taddr_hi, uint32_t taddr_lo, const float (&x)[16]) {
-  uint32_t hi[16], lo[16];
-#pragma unroll
-  for (int i = 0; i < 16; ++i) {
-    split_tf32(x[i], hi[i], lo[i]);
-  }
-  tmem_st16(taddr_hi, hi);
-  tmem_st16(taddr_lo, lo);
-}
-
-// ---- UMMA descriptors --------------------------------------------------------------------------------------
+// ---- shared-memory operand tiles + warpgroup MMA (wgmma) -------------------------------------------------------
 // K-major operand tile [rows][32 tf32] in SWIZZLE_128B layout: row r at (r/8)*1024 + (r%8)*128 bytes, the
-// eight 16-byte chunks of a row XOR-ed with (r%8).  SBO = 1024 B (8-row groups), LBO unused, version 1.
-__device__ __forceinline__ uint64_t smem_desc_sw128(const void* tile) {
-  const uint64_t addr = (uint64_t)(smem_u32(tile) >> 4) & 0x3FFFull;
-  return addr | (0ull << 16) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 46) | (2ull << 61);
-}
-// instruction descriptor: D=F32, A=B=TF32, both K-major, shape M x N
-__host__ __device__ constexpr uint32_t idesc_tf32(uint32_t M, uint32_t N) {
-  return (1u << 4) | (2u << 7) | (2u << 10) | ((N >> 3) << 17) | ((M >> 4) << 24);
-}
-// byte offset of element (row, k) inside a swizzled [rows][32] tile
+// eight 16-byte chunks of a row XOR-ed with (r%8).  Tiles start on a 1024-byte boundary.
 __host__ __device__ inline uint32_t sw128_offset(uint32_t row, uint32_t k) {
   return (row >> 3) * 1024u + (row & 7u) * 128u + ((((k >> 2) ^ row) & 7u) << 4) + ((k & 3u) << 2);
 }
-
-// D[tmem_d] (+)= A[tmem_a : 128 lanes x 8 cols tf32] * B[smem desc : N rows x 8 tf32]^T   (one elected thread)
-__device__ __forceinline__ void mma_tf32_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], [%1], %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "r"(tmem_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
+// wgmma shared-memory descriptor of such a tile: start address >> 4, LBO unused (16 B), SBO = 1024 B between
+// 8-row groups, layout type 1 = SWIZZLE_128B.  Advancing the start address by 32 B (+2) selects the next 8-deep k-step.
+__device__ __forceinline__ uint64_t smem_desc_sw128(const void* tile) {
+  const uint64_t addr = (uint64_t)(smem_u32(tile) >> 4) & 0x3FFFull;
+  return addr | (1ull << 16) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 62);
 }
-// same with BOTH operands in shared memory (A: 128 rows x 8 tf32 K-major tile, same descriptor format as B)
-__device__ __forceinline__ void mma_tf32_ss(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
+// 8 consecutive k of one row: hi tile and lo tile (3xTF32 split of x)
+__device__ __forceinline__ void st_hilo8(uint8_t* tile_hi, uint8_t* tile_lo, uint32_t row, uint32_t k0, const float (&x)[8]) {
+  float h[8], l[8];
+#pragma unroll
+  for (int i = 0; i < 8; ++i) split_tf32(x[i], h[i], l[i]);
+#pragma unroll
+  for (int c = 0; c < 2; ++c) {
+    const uint32_t off = sw128_offset(row, k0 + 4 * c);
+    *reinterpret_cast<float4*>(tile_hi + off) = make_float4(h[4 * c], h[4 * c + 1], h[4 * c + 2], h[4 * c + 3]);
+    *reinterpret_cast<float4*>(tile_lo + off) = make_float4(l[4 * c], l[4 * c + 1], l[4 * c + 2], l[4 * c + 3]);
+  }
 }
 // operand tiles written with ordinary st.shared must be made visible to the async proxy (tensor core reads)
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-// all previously issued MMAs of this thread arrive on the mbarrier when complete
-__device__ __forceinline__ void mma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
+
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+
+// D[64 x N] (+)= A[64 rows x 8 tf32, smem desc] * B[N rows x 8 tf32, smem desc]^T, issued by one whole warpgroup.
+// Accumulator fragment (N/2 floats per thread): d[4j + {0,1}] = row 16*warp + lane/4, columns 8j + 2*(lane%4) + {0,1};
+// d[4j + {2,3}] = the same columns of row + 8.
+__device__ __forceinline__ void wgmma_tf32_n64(float* d, uint64_t da, uint64_t db, uint32_t acc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(da), "l"(db), "r"(acc));
+}
+__device__ __forceinline__ void wgmma_tf32_n128(float* d, uint64_t da, uint64_t db, uint32_t acc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, %64, %65, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(da), "l"(db), "r"(acc));
+}
+__device__ __forceinline__ void wgmma_tf32_n192(float* d, uint64_t da, uint64_t db, uint32_t acc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %98, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n192k8.f32.tf32.tf32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63,%64,%65,%66,%67,%68,%69,%70,%71,%72,%73,%74,%75,%76,%77,%78,%79,%80,%81,%82,%83,%84,%85,%86,%87,%88,%89,%90,%91,%92,%93,%94,%95}, %96, %97, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]), "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95])
+      : "l"(da), "l"(db), "r"(acc));
+}
+__device__ __forceinline__ void wgmma_tf32_n256(float* d, uint64_t da, uint64_t db, uint32_t acc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %130, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n256k8.f32.tf32.tf32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63,%64,%65,%66,%67,%68,%69,%70,%71,%72,%73,%74,%75,%76,%77,%78,%79,%80,%81,%82,%83,%84,%85,%86,%87,%88,%89,%90,%91,%92,%93,%94,%95,%96,%97,%98,%99,%100,%101,%102,%103,%104,%105,%106,%107,%108,%109,%110,%111,%112,%113,%114,%115,%116,%117,%118,%119,%120,%121,%122,%123,%124,%125,%126,%127}, %128, %129, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]), "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]), "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]), "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]), "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]), "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+      : "l"(da), "l"(db), "r"(acc));
+}
+__device__ __forceinline__ void wgmma_tf32(int N, float* d, uint64_t da, uint64_t db, uint32_t acc) {
+  switch (N) {
+    case 64: wgmma_tf32_n64(d, da, db, acc); break;
+    case 128: wgmma_tf32_n128(d, da, db, acc); break;
+    case 192: wgmma_tf32_n192(d, da, db, acc); break;
+    default: wgmma_tf32_n256(d, da, db, acc); break;
+  }
+}
+// one 32-deep k-block of a 3xTF32 GEMM: a_hi*b_hi + a_hi*b_lo + a_lo*b_hi per 8-deep k-step
+__device__ __forceinline__ void wgmma_kblock_3x(int N, float* d, uint64_t a_hi, uint64_t a_lo, uint64_t b_hi, uint64_t b_lo,
+                                                int ksteps, bool first) {
+  for (int ks = 0; ks < ksteps; ++ks) {
+    wgmma_tf32(N, d, a_hi + 2 * ks, b_hi + 2 * ks, (first && ks == 0) ? 0u : 1u);
+    wgmma_tf32(N, d, a_hi + 2 * ks, b_lo + 2 * ks, 1u);
+    wgmma_tf32(N, d, a_lo + 2 * ks, b_hi + 2 * ks, 1u);
+  }
 }
 
 }  // namespace tc

@@ -1,9 +1,9 @@
-// tc_bwd.cu -- tcgen05 version of one reverse BPTT step of the cell (K9): gate derivatives on CUDA
+// tc_bwd.cu -- tensor-core (wgmma) version of one reverse BPTT step of the cell (K9): gate derivatives on CUDA
 // cores, then the dgrad GEMM  d[s | h^] = dz [wx;wh]^T  and the message-gradient GEMM
-// dm = dpre_m W_msg^T  as 3xTF32 tcgen05.mma with the A operand (dz, dpre_m) written straight from
-// registers into TMEM and the pre-packed transposed weights bulk-copied into swizzled shared memory.
-// Same CTA structure as tc_cell.cu (128 env rows x one agent, 4 warp-sets of row threads + producer +
-// MMA issuer); same inputs/outputs as cell_bwd_kernel (train.cu).
+// dm = dpre_m W_msg^T  as 3xTF32 wgmma with the A operand (dz, dpre_m) written from registers into the
+// swizzled shared-memory ring and the pre-packed transposed weights bulk-copied into swizzled shared memory.
+// Same CTA structure as tc_cell.cu (64 env rows x one agent, 4 warp-sets of row threads + MMA warpgroup +
+// producer); same inputs/outputs as cell_bwd_kernel (train.cu).
 #include "bwd_common.cuh"
 #include "tc_row.cuh"
 
@@ -16,19 +16,12 @@ template <int VAR, bool FM, bool RAW>
 __global__ void __launch_bounds__(TC_THREADS, 1) tc_cell_bwd_kernel(const __grid_constant__ nmarl_model m,
                                                                     const __grid_constant__ BwdK k) {
   extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* bst = smem;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + S_STAGES * STAGE_BYTES);
-  uint64_t* b_full = bars, *b_empty = bars + S_STAGES, *a_full = bars + 2 * S_STAGES, *a_empty = a_full + A_SLOTS;
-  uint64_t* enc_full = a_empty + A_SLOTS, *acc_full = enc_full + 1;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_full + 1);
-  int* n_kb_s = reinterpret_cast<int*>(tmem_slot + 1);
-  KbEnt* sched = reinterpret_cast<KbEnt*>(tmem_slot + 4);
-  float* bsum = reinterpret_cast<float*>(sched + MAX_KB);         // [4 quarters][256] gate-bias partial sums
+  const Smem sm = smem_map(smem_raw);
+  KbEnt* sched = sm.sched;
 
   const int i = blockIdx.y;
   const nmarl_agent& ag = m.agent[i];
-  const int B = k.B, b0 = blockIdx.x * 128;
+  const int B = k.B, b0 = blockIdx.x * ROWS;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int n_a = m.n_a, SD = m.s_dim;
   const float* __restrict__ P = k.params;
@@ -36,11 +29,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_cell_bwd_kernel(const __grid
   const int Km = (VAR == NMARL_IC3) ? NH : ag.n_nbr * NH;
 
   if (tid == 0) {
-    for (int s = 0; s < S_STAGES; ++s) { tc::mbar_init(&b_full[s], 1); tc::mbar_init(&b_empty[s], 1); }
-    for (int s = 0; s < A_SLOTS; ++s) { tc::mbar_init(&a_full[s], ROW_THREADS); tc::mbar_init(&a_empty[s], 1); }
-    tc::mbar_init(enc_full, 1);
-    tc::mbar_init(acc_full, 1);
-    tc::fence_barrier_init();
+    init_barriers(sm);
     int n = 0;
     // dgrad k-blocks in the order the row threads produce dz: gate o first (its inputs are already in registers from
     // the dc computation), then i and u (which share their two loads), then f
@@ -48,22 +37,18 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_cell_bwd_kernel(const __grid
     for (int q = 0; q < 8; ++q) sched[n++] = make_kb(ag.tp_gT, SD + NH, NG, korder[q], 0, q == 0, 0, q == 7);
     if (VAR != NMARL_IA2C && Km > 0)
       for (int kb = 0; kb < 2; ++kb) sched[n++] = make_kb(ag.tp_mT, Km, NH, kb, 0, kb == 0, 0, kb == 1);
-    *n_kb_s = n;
+    *sm.n_kb = n;
   }
-  if (warp == ROW_THREADS / 32 + 1) tc::tmem_alloc(tmem_slot, 512);
-  tc::fence_before_sync();
   __syncthreads();
-  tc::fence_after_sync();
-  const uint32_t tmem = *tmem_slot;
-  const int n_kb = *n_kb_s;
+  const int n_kb = *sm.n_kb;
   tc::pdl_launch_dependents();       // PDL (tc.cuh): the prologue overlapped the previous reverse step's tail
   tc::pdl_wait();
 
-  if (warp < ROW_THREADS / 32) {
+  if (warp < MMA_WARP0) {
     RowCtx c;
-    const int set = warp >> 2, quarter = warp & 3, r = quarter * 32 + lane;
-    c.tmem = tmem; c.lane_base = (uint32_t)(quarter * 32) << 16;
-    c.a_full = a_full; c.a_empty = a_empty; c.enc_full = enc_full; c.q = 0; c.e = 0; c.set = set; c.err = k.tc_err;
+    const int set = warp / ROW_WARPS, rh = warp % ROW_WARPS, r = rh * 32 + lane;
+    c.a_ring = sm.ast; c.acc = sm.acc; c.r = (uint32_t)r;
+    c.a_full = sm.a_full; c.a_empty = sm.a_empty; c.enc_full = sm.enc_full; c.q = 0; c.e = 0; c.set = set; c.err = k.tc_err;
     const int b = b0 + r;
     const size_t row = (size_t)i * B + b;
     const float nd = 1.0f - k.done_pre[b];
@@ -128,7 +113,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_cell_bwd_kernel(const __grid
     // two dgrad A k-blocks.  Order o, i, u, f (see the k-block schedule above): every saved gate is loaded once.
     auto emit = [&](const int g, const float (&dz)[EW]) {
       {   // gate-bias gradient = column sums of dz: sum over this warp's 32 rows by recursive halving (16 shuffles per
-          // gate instead of a feature-major copy of dz in HBM + a separate column-sum kernel)
+          // gate instead of a feature-major copy of dz in HBM + a separate column-sum kernel); one partial per 32 rows
         float a[EW];
 #pragma unroll
         for (int j = 0; j < EW; ++j) a[j] = dz[j];
@@ -144,10 +129,10 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_cell_bwd_kernel(const __grid
         }
         a[0] += __shfl_xor_sync(0xffffffffu, a[0], 1);
         const int col = (((lane >> 4) & 1) << 3) | (((lane >> 3) & 1) << 2) | (((lane >> 2) & 1) << 1) | ((lane >> 1) & 1);
-        if ((lane & 1) == 0) bsum[quarter * NG + g * NH + e0 + col] = a[0];
+        if ((lane & 1) == 0) k.sv_dz[((size_t)i * (B / 32) + (b0 / 32) + rh) * NG + g * NH + e0 + col] = a[0];
       }
       if (k.dzT != nullptr) {                 // dz^T tile for the tensor-core wgrad: K-major over rows, hi | lo
-        uint8_t* tile = reinterpret_cast<uint8_t*>(k.dzT) + ((size_t)i * (B / 32) + (b0 / 32) + quarter) * (size_t)((RAW ? 1 : 2) * 256 * 128);
+        uint8_t* tile = reinterpret_cast<uint8_t*>(k.dzT) + ((size_t)i * (B / 32) + (b0 / 32) + rh) * (size_t)((RAW ? 1 : 2) * 256 * 128);
 #pragma unroll
         for (int j = 0; j < EW; ++j) {
           const uint32_t off = tc::sw128_offset((uint32_t)(g * NH + e0 + j), (uint32_t)lane);
@@ -188,20 +173,13 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_cell_bwd_kernel(const __grid
       emit(1, dz);
     }
 
-    // per-tile gate-bias partial sums (fixed order over the four row quarters), reduced over (t, tile) afterwards
-    row_barrier();
-    if (tid < NG) {
-      const float sm = ((bsum[tid] + bsum[NG + tid]) + bsum[2 * NG + tid]) + bsum[3 * NG + tid];
-      k.sv_dz[((size_t)i * gridDim.x + blockIdx.x) * NG + tid] = sm;
-    }
     // ---- dgrad result: d[s | h^] -------------------------------------------------------------------------------
-    tc::mbar_wait(acc_full, 0, k.tc_err, 13);
-    tc::fence_after_sync();
+    tc::mbar_wait(sm.acc_full, 0, k.tc_err, 13);
     float dpm[EW];
 #pragma unroll
     for (int j = 0; j < EW; ++j) dpm[j] = 0.f;
     uint8_t* dptile = (k.dpT != nullptr)
-        ? reinterpret_cast<uint8_t*>(k.dpT) + ((size_t)i * (B / 32) + (b0 / 32) + quarter) * (size_t)((RAW ? 1 : 2) * k.ndp * 128) : nullptr;
+        ? reinterpret_cast<uint8_t*>(k.dpT) + ((size_t)i * (B / 32) + (b0 / 32) + rh) * (size_t)((RAW ? 1 : 2) * k.ndp * 128) : nullptr;
     auto put_dp = [&](int n0, const float (&vals)[EW]) {        // encoder pre-activation grads as K-major tiles
       if (dptile == nullptr) return;
 #pragma unroll
@@ -223,8 +201,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_cell_bwd_kernel(const __grid
 #pragma unroll
       for (int p = 0; p < EW / 8; ++p) {
         float t[8];
-        tc::tmem_ld8(tmem + c.lane_base + ACC_COL + gp * NH + e0 + 8 * p, t);
-        tc::wait_ld();
+        acc_ld8(c, ACC_COL + gp * NH + e0 + 8 * p, t);
 #pragma unroll
         for (int j = 0; j < 8; ++j) d[8 * p + j] = t[j];
       }
@@ -255,20 +232,17 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_cell_bwd_kernel(const __grid
         put_dp(NH + e0, dpm);
       }
     }
-    tc::fence_before_sync();
     // ---- message gradient dm = dpre_m W_msg^T, one 64-wide block per neighbour slot --------------------------
     if (VAR != NMARL_IA2C && Km > 0) {
       produce_act(c, dpm);
-      tc::mbar_wait(acc_full, 1, k.tc_err, 14);
-      tc::fence_after_sync();
+      tc::mbar_wait(sm.acc_full, 1, k.tc_err, 14);
       const int nblk = (VAR == NMARL_IC3) ? 1 : ag.n_nbr;
       for (int s = 0; s < nblk; ++s) {
         float d[EW];
 #pragma unroll
         for (int p = 0; p < EW / 8; ++p) {
           float t[8];
-          tc::tmem_ld8(tmem + c.lane_base + ACC_COL + s * NH + e0 + 8 * p, t);
-          tc::wait_ld();
+          acc_ld8(c, ACC_COL + s * NH + e0 + 8 * p, t);
 #pragma unroll
           for (int j = 0; j < 8; ++j) d[8 * p + j] = t[j];
         }
@@ -281,15 +255,10 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_cell_bwd_kernel(const __grid
           st_state<FM, EW>(k.dmsg_out, (size_t)i * NMARL_MAX_NBR + s, b, e0, B, d);
         }
       }
-      tc::fence_before_sync();
     }
-  } else if (warp == ROW_THREADS / 32) {
-    if (tc::elect_one()) producer_loop(sched, n_kb, bst, b_full, b_empty, k.wpack, k.tc_err);
   } else {
-    if (tc::elect_one()) mma_loop(sched, n_kb, bst, b_full, b_empty, a_full, a_empty, enc_full, acc_full, tmem, k.tc_err);
+    mma_loop(sched, n_kb, sm.bst, sm.ast, sm.b_full, sm.a_full, sm.a_empty, sm.enc_full, sm.acc_full, sm.acc, k.wpack, k.tc_err);
   }
-  __syncthreads();
-  if (warp == ROW_THREADS / 32 + 1) { tc::fence_after_sync(); tc::tmem_dealloc(tmem, 512); }
 }
 
 template <int VAR, bool FM, bool RAW>
@@ -300,7 +269,7 @@ int launch_tc_bwd_fm(const nmarl_model* m, const BwdK& k, cudaStream_t st) {
     NMARL_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TC_SMEM));
     configured = true;
   }
-  dim3 grid(k.B / 128, m->n_agent);
+  dim3 grid(k.B / ROWS, m->n_agent);
   NMARL_CUDA(nmarl_launch(kern, grid, dim3(TC_THREADS), TC_SMEM, st, true, *m, k));
   NMARL_LAUNCH_CHECK();
   return 0;

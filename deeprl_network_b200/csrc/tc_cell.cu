@@ -1,20 +1,19 @@
-// tc_cell.cu -- tcgen05 (5th-gen tensor core) version of the fused forward cell (K2..K6):
+// tc_cell.cu -- tensor-core (wgmma) version of the fused forward cell (K2..K6):
 // every GEMM of the step (obs / fingerprint / message encoders and the LSTM gate GEMM) runs as
-// 3xTF32 tcgen05.mma with FP32 accumulators in TMEM; CUDA cores only do the elementwise epilogues.
+// 3xTF32 wgmma with FP32 accumulators; CUDA cores only do the gathers and the elementwise epilogues.
 //
-// One CTA = 128 envs of one agent (UMMA M = 128).  576 threads:
-//   warps 0-15 "row threads": 4 warp-sets x 4 warps; a thread of set s in TMEM-lane quarter w owns env
-//              row r = 32 w + lane (TMEM lane r) and the column slice s of it.  They gather the row's
-//              inputs, split them hi/lo and tcgen05.st them as the A operand (A lives in TMEM, so no
-//              shared memory is spent on activations), read encoder results back with tcgen05.ld, apply
-//              bias/activation, feed them to the gate GEMM, and finally run the LSTM cell update, the
-//              heads, softmax and sampling for their row.
-//   warp 16    B producer: one cp.async.bulk (TMA engine) per 32-wide k-block of pre-packed,
-//              128B-swizzled [hi | lo] weight tiles into a 3-stage shared-memory ring (mbarrier tx).
-//   warp 17    MMA issuer: a single elected thread issues tcgen05.mma kind::tf32 (3 per k-step:
-//              hi*hi + hi*lo + lo*hi) and tcgen05.commit's completion onto the ring barriers.
-// TMEM (512 columns): [0,256) accumulators (the encoder GEMMs land in 64-column blocks of it and are consumed
-// before the gate GEMM overwrites it), [256,512) A-operand ring (4 slots x (hi 32 | lo 32)).
+// One CTA = 64 envs of one agent (wgmma M = 64).  384 threads:
+//   warps 0-7  "row threads": 4 warp-sets x 2 warps; a thread of set s in warp half h owns env row
+//              r = 32 h + lane and the column slice s of it.  They gather the row's inputs, split them hi/lo
+//              and store them as the A operand (a 128B-swizzled shared-memory ring), read the finished GEMM
+//              results back from the accumulator staging area, apply bias/activation, feed them to the gate
+//              GEMM, and finally run the LSTM cell update, the heads, softmax and sampling for their row.
+//   warps 8-11 MMA warpgroup: 3 wgmma per 8-deep k-step (hi*hi + hi*lo + lo*hi) into a register accumulator;
+//              each finished GEMM is stored to the staging area (tc_row.cuh).  Its thread 0 also streams the
+//              pre-packed, 128B-swizzled [hi | lo] weight tiles, one cp.async.bulk (TMA engine) per 32-wide
+//              k-block, into a 2-stage shared-memory ring (mbarrier tx).
+// Staging area (64 rows x 256 columns): the encoder GEMMs land in 64-column blocks of it and are consumed before
+// the gate GEMM overwrites it.
 //
 // Same math, same argument block and same outputs as cell_fwd.cu (FP32 FFMA); used when
 // B % 128 == 0 and packed weights are supplied.  Restates the same reference lines as cell_fwd.cu.
@@ -33,32 +32,21 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_cell_fwd_kernel(const __grid
   constexpr bool SAVE = (MODE == MODE_TRAIN || MODE == MODE_PS);   // store activations for BPTT
   constexpr bool SAMPLE = (MODE == MODE_P || MODE == MODE_PS);     // p-call: sample actions
   extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* bst = smem;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + S_STAGES * STAGE_BYTES);
-  uint64_t* b_full = bars, *b_empty = bars + S_STAGES, *a_full = bars + 2 * S_STAGES, *a_empty = a_full + A_SLOTS;
-  uint64_t* enc_full = a_empty + A_SLOTS, *acc_full = enc_full + 1;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_full + 1);
-  int* n_kb_s = reinterpret_cast<int*>(tmem_slot + 1);
-  KbEnt* sched = reinterpret_cast<KbEnt*>(tmem_slot + 4);
-  float* hpart = reinterpret_cast<float*>(sched + MAX_KB);       // [NSET][128][8] head partial sums
-  __shared__ float red[3][4];
+  const Smem sm = smem_map(smem_raw);
+  KbEnt* sched = sm.sched;
+  __shared__ float red[3][ROW_WARPS];
 
   const nmarl_fwd_args& a = k.a;
   const int i = blockIdx.y;
   const nmarl_agent& ag = m.agent[i];
-  const int B = a.B, b0 = blockIdx.x * 128;
+  const int B = a.B, b0 = blockIdx.x * ROWS;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int n_a = m.n_a, SD = m.s_dim;
   const float* __restrict__ P = a.params;
   const int Kx = ag.x_nsrc * ag.x_w;
 
   if (tid == 0) {
-    for (int s = 0; s < S_STAGES; ++s) { tc::mbar_init(&b_full[s], 1); tc::mbar_init(&b_empty[s], 1); }
-    for (int s = 0; s < A_SLOTS; ++s) { tc::mbar_init(&a_full[s], ROW_THREADS); tc::mbar_init(&a_empty[s], 1); }
-    tc::mbar_init(enc_full, 1);
-    tc::mbar_init(acc_full, 1);
-    tc::fence_barrier_init();
+    init_barriers(sm);
     // ---- k-block schedule shared by the three roles: all encoder GEMMs first (each into its own 64-column
     // block of the accumulator region, one completion barrier), then the gate GEMM over [s | h^] ----------------
     int n = 0;
@@ -74,25 +62,21 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_cell_fwd_kernel(const __grid
     for (int g = 0; g < nG; ++g) sched[n++] = make_kb(ag.tp_g, 256, KG, g, ACC_COL, g == 0, 0, g == nG - 1);
     if (VAR == NMARL_DIAL && MODE != MODE_V)
       for (int j = 0; j < 2; ++j) sched[n++] = make_kb(ag.tp_mfc, 64, NH, j, ACC_COL, j == 0, j == 1, 0);
-    *n_kb_s = n;
+    *sm.n_kb = n;
   }
-  if (warp == ROW_THREADS / 32 + 1) tc::tmem_alloc(tmem_slot, 512);
-  tc::fence_before_sync();
   __syncthreads();
-  tc::fence_after_sync();
-  const uint32_t tmem = *tmem_slot;
-  const int n_kb = *n_kb_s;
+  const int n_kb = *sm.n_kb;
   // PDL: the prologue above overlapped the tail of the previous kernel of the stream; from here on the kernel reads
   // what that kernel (env step / previous cell call) wrote.
   tc::pdl_launch_dependents();
   tc::pdl_wait();
 
-  if (warp < ROW_THREADS / 32) {
+  if (warp < MMA_WARP0) {
     // =================================== row threads ===================================================
     RowCtx c;
-    const int set = warp >> 2, quarter = warp & 3, r = quarter * 32 + lane;
-    c.tmem = tmem; c.lane_base = (uint32_t)(quarter * 32) << 16;
-    c.a_full = a_full; c.a_empty = a_empty; c.enc_full = enc_full; c.q = 0; c.e = 0; c.set = set; c.err = a.tc_err;
+    const int set = warp / ROW_WARPS, rh = warp % ROW_WARPS, r = rh * 32 + lane;
+    c.a_ring = sm.ast; c.acc = sm.acc; c.r = (uint32_t)r;
+    c.a_full = sm.a_full; c.a_empty = sm.a_empty; c.enc_full = sm.enc_full; c.q = 0; c.e = 0; c.set = set; c.err = a.tc_err;
     const int b = b0 + r;
     const size_t row = (size_t)i * B + b;
     const float nd = 1.0f - a.done[b];
@@ -261,8 +245,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_cell_fwd_kernel(const __grid
     }
     STAMP();
     // ---- LSTM cell update for hidden units [e0, e0 + EW), 8 at a time; partial head sums -----------------------
-    tc::mbar_wait(acc_full, 0, a.tc_err, 13);
-    tc::fence_after_sync();
+    tc::mbar_wait(sm.acc_full, 0, a.tc_err, 13);
     STAMP();
     float logit[NMARL_MAX_NA];
 #pragma unroll
@@ -271,11 +254,10 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_cell_fwd_kernel(const __grid
 #pragma unroll 1
     for (int u0 = e0; u0 < e0 + EW; u0 += 8) {
       float gi[8], gf[8], go[8], gu[8];
-      tc::tmem_ld8(tmem + c.lane_base + ACC_COL + 0 * NH + u0, gi);
-      tc::tmem_ld8(tmem + c.lane_base + ACC_COL + 1 * NH + u0, gf);
-      tc::tmem_ld8(tmem + c.lane_base + ACC_COL + 2 * NH + u0, go);
-      tc::tmem_ld8(tmem + c.lane_base + ACC_COL + 3 * NH + u0, gu);
-      tc::wait_ld();
+      acc_ld8(c, ACC_COL + 0 * NH + u0, gi);
+      acc_ld8(c, ACC_COL + 1 * NH + u0, gf);
+      acc_ld8(c, ACC_COL + 2 * NH + u0, go);
+      acc_ld8(c, ACC_COL + 3 * NH + u0, gu);
       STAMP();
       float cn[8], hn[8], cpv[8];
       ld_state<FM, 8>(a.c_in, (size_t)i, b, u0, B, cpv);
@@ -346,15 +328,16 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_cell_fwd_kernel(const __grid
         for (int x = 0; x < 8; ++x) s0[(u0 - e0) + x] = hn[x];
       }
     }
-    tc::fence_before_sync();
     if (VAR == NMARL_DIAL && MODE != MODE_V) produce_act(c, s0);
 
     // ---- heads: combine the NSET partial sums of a row in fixed order, then softmax / sampling / loss -------
+    // The partial sums of set s go to staging columns [NH + s*EW, +8) of the row: gate-f cells that only this
+    // thread has read, and that the DIAL message GEMM (columns [0, NH)) does not overwrite.
     {
-      float* hp = hpart + ((size_t)set * 128 + r) * 8;
+      float* hp = sm.acc;
 #pragma unroll
-      for (int cc = 0; cc < NMARL_MAX_NA - 1; ++cc) hp[cc] = logit[cc];
-      hp[NMARL_MAX_NA - 1] = v;
+      for (int cc = 0; cc < NMARL_MAX_NA - 1; ++cc) hp[acc_idx(r, NH + e0 + cc)] = logit[cc];
+      hp[acc_idx(r, NH + e0 + NMARL_MAX_NA - 1)] = v;
     }
     STAMP();
     row_barrier();
@@ -366,10 +349,10 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_cell_fwd_kernel(const __grid
       v = 0.f;
 #pragma unroll
       for (int s = 0; s < NSET; ++s) {
-        const float* hp = hpart + ((size_t)s * 128 + r) * 8;
+        const float* hp = sm.acc;
 #pragma unroll
-        for (int cc = 0; cc < NMARL_MAX_NA - 1; ++cc) logit[cc] += hp[cc];
-        v += hp[NMARL_MAX_NA - 1];
+        for (int cc = 0; cc < NMARL_MAX_NA - 1; ++cc) logit[cc] += hp[acc_idx(r, NH + s * EW + cc)];
+        v += hp[acc_idx(r, NH + s * EW + NMARL_MAX_NA - 1)];
       }
       float pi[NMARL_MAX_NA];
       if (MODE != MODE_V) {
@@ -464,25 +447,18 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_cell_fwd_kernel(const __grid
       for (int cc = 0; cc < 3; ++cc) {
         float x = vals[cc];
         for (int o = 16; o > 0; o >>= 1) x += __shfl_xor_sync(0xffffffffu, x, o);
-        if (lane == 0) red[cc][quarter] = x;
+        if (lane == 0) red[cc][rh] = x;
       }
     }
-  } else if (warp == ROW_THREADS / 32) {
-    // =================================== B producer ======================================================
-    if (tc::elect_one()) producer_loop(sched, n_kb, bst, b_full, b_empty, a.wpack, a.tc_err);
   } else {
-    // =================================== MMA issuer ======================================================
-    if (tc::elect_one()) mma_loop(sched, n_kb, bst, b_full, b_empty, a_full, a_empty, enc_full, acc_full, tmem, a.tc_err,
-                            (k.prof != nullptr && blockIdx.x == 0 && blockIdx.y == 1) ? k.prof : nullptr);
+    // =================================== MMA warpgroup ===================================================
+    mma_loop(sched, n_kb, sm.bst, sm.ast, sm.b_full, sm.a_full, sm.a_empty, sm.enc_full, sm.acc_full, sm.acc, a.wpack, a.tc_err);
   }
   __syncthreads();
   if (MODE == MODE_TRAIN && tid < 3) {
-    const float s = ((red[tid][0] + red[tid][1]) + red[tid][2]) + red[tid][3];
-    float* lp = k.loss_part + ((size_t)i * k.loss_tiles + 2 * blockIdx.x) * 4;
-    lp[tid] = s;
-    lp[4 + tid] = 0.f;                 // the second 64-row slot of this 128-row tile
+    static_assert(ROWS == 64 && ROW_WARPS == 2, "one 64-row loss tile per CTA");
+    k.loss_part[((size_t)i * k.loss_tiles + blockIdx.x) * 4 + tid] = red[tid][0] + red[tid][1];
   }
-  if (warp == ROW_THREADS / 32 + 1) { tc::fence_after_sync(); tc::tmem_dealloc(tmem, 512); }
 }
 
 
@@ -494,7 +470,7 @@ int launch_tc_fm(const nmarl_model* m, const FwdK& k, cudaStream_t st) {
     NMARL_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TC_SMEM));
     configured = true;
   }
-  dim3 grid(k.a.B / 128, m->n_agent);
+  dim3 grid(k.a.B / ROWS, m->n_agent);
   FwdK k2 = k;
   k2.prof = g_nmarl_prof;
   NMARL_CUDA(nmarl_launch(kern, grid, dim3(TC_THREADS), TC_SMEM, st, true, *m, k2));

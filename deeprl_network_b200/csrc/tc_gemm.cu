@@ -1,5 +1,5 @@
-// tc_gemm.cu -- weight packing for the tcgen05 path + a stand-alone 3xTF32 GEMM used by the tests to
-// validate the tensor-core pipeline (TMEM alloc, tcgen05.st/ld, UMMA descriptors, bulk copies, mbarriers)
+// tc_gemm.cu -- weight packing for the tensor-core path + a stand-alone 3xTF32 GEMM used by the tests to
+// validate the tensor-core pipeline (swizzled operand tiles, wgmma descriptors, bulk copies, mbarriers)
 // in isolation:  C[M x N] = A[M x K] * W[K x N]   (M % 128 == 0, K % 8 == 0, N in {64, 256}).
 #include "common.cuh"
 #include "tc.cuh"
@@ -44,172 +44,81 @@ __global__ void pack_b_raw_kernel(const float* __restrict__ W, int ldw, int K, i
   }
 }
 
+// 64 rows per CTA: warps 0-3 are the MMA warpgroup (accumulator in registers, written straight to C), warps 4-5
+// produce the A operand (one row per thread) into the swizzled shared-memory ring, warp 6 bulk-copies B.
 template <int N>
-__global__ void __launch_bounds__(192, 1) tc_gemm_test_kernel(const float* __restrict__ A, int K, const float* __restrict__ Bp,
+__global__ void __launch_bounds__(224, 1) tc_gemm_test_kernel(const float* __restrict__ A, int K, const float* __restrict__ Bp,
                                                               float* __restrict__ C, int* err) {
-  constexpr int S = 2;                                   // B stages
-  constexpr uint32_t TILE = N * 128;                     // bytes of one hi (or lo) tile
+  constexpr int S = 2;                                   // B stages and A slots
+  constexpr uint32_t TILE = N * 128;                     // bytes of one hi (or lo) B tile
   constexpr uint32_t STAGE = 2 * TILE;
-  constexpr uint32_t ACC_COL = 0, A_COL = 256;           // TMEM columns: accumulator, then 2 x (hi32 | lo32)
+  constexpr uint32_t A_TILE = 64 * 128, A_SLOT = 2 * A_TILE;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* bst = smem;                                   // S stages
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + S * STAGE);
-  uint64_t* b_full = bars, *b_empty = bars + S, *a_full = bars + 2 * S, *a_empty = bars + 2 * S + 2, *acc_full = bars + 2 * S + 4;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * S + 5);
+  uint8_t* bst = smem;
+  uint8_t* ast = smem + S * STAGE;
+  uint64_t* bars = reinterpret_cast<uint64_t*>(ast + S * A_SLOT);
+  uint64_t* b_full = bars, *b_empty = bars + S, *a_full = bars + 2 * S, *a_empty = bars + 3 * S;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int nkb = (K + 31) / 32;
   if (tid == 0) {
-    for (int s = 0; s < S; ++s) { tc::mbar_init(&b_full[s], 1); tc::mbar_init(&b_empty[s], 1); }
-    for (int s = 0; s < 2; ++s) { tc::mbar_init(&a_full[s], 128); tc::mbar_init(&a_empty[s], 1); }
-    tc::mbar_init(acc_full, 1);
+    for (int s = 0; s < S; ++s) {
+      tc::mbar_init(&b_full[s], 1); tc::mbar_init(&b_empty[s], 128);
+      tc::mbar_init(&a_full[s], 64); tc::mbar_init(&a_empty[s], 128);
+    }
     tc::fence_barrier_init();
   }
-  if (warp == 5) tc::tmem_alloc(tmem_slot, 512);
-  tc::fence_before_sync();
   __syncthreads();
-  tc::fence_after_sync();
-  const uint32_t tmem = *tmem_slot;
 
   if (warp < 4) {
-    // ---- row threads: produce the A operand chunks, then the epilogue ----
-    const size_t row = (size_t)blockIdx.x * 128 + tid;
-    const uint32_t lane_base = (uint32_t)(warp * 32) << 16;
+    float d[N / 2];
+#pragma unroll
+    for (int j = 0; j < N / 2; ++j) d[j] = 0.f;
     for (int kb = 0; kb < nkb; ++kb) {
-      const int slot = kb & 1;
-      tc::mbar_wait(&a_empty[slot], ((kb >> 1) & 1) ^ 1, err, 1);
-      tc::fence_after_sync();
+      const int st = kb % S;
+      tc::mbar_wait(&b_full[st], (kb / S) & 1, err, 4);
+      tc::mbar_wait(&a_full[st], (kb / S) & 1, err, 5);
+      const int ksteps = min(4, (K - kb * 32) / 8);
+      uint8_t* a = ast + st * A_SLOT;
+      uint8_t* b = bst + st * STAGE;
+      tc::wgmma_fence();
+      tc::wgmma_kblock_3x(N, d, tc::smem_desc_sw128(a), tc::smem_desc_sw128(a + A_TILE), tc::smem_desc_sw128(b),
+                          tc::smem_desc_sw128(b + TILE), ksteps, kb == 0);
+      tc::wgmma_commit();
+      tc::wgmma_wait_all();
+      tc::mbar_arrive(&a_empty[st]);
+      tc::mbar_arrive(&b_empty[st]);
+    }
+    const size_t r0 = (size_t)blockIdx.x * 64 + 16 * warp + (lane >> 2);
 #pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        float x[16];
+    for (int j = 0; j < N / 8; ++j) {
+      const int col = 8 * j + 2 * (lane & 3);
+      *reinterpret_cast<float2*>(C + r0 * N + col) = make_float2(d[4 * j], d[4 * j + 1]);
+      *reinterpret_cast<float2*>(C + (r0 + 8) * N + col) = make_float2(d[4 * j + 2], d[4 * j + 3]);
+    }
+  } else if (warp < 6) {
+    const int r = tid - 128;
+    const size_t row = (size_t)blockIdx.x * 64 + r;
+    for (int kb = 0; kb < nkb; ++kb) {
+      const int st = kb % S;
+      tc::mbar_wait(&a_empty[st], ((kb / S) & 1) ^ 1, err, 1);
+      uint8_t* hi = ast + st * A_SLOT;
 #pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          const int k = kb * 32 + h * 16 + q * 4;
+      for (int h = 0; h < 4; ++h) {
+        float x[8];
+#pragma unroll
+        for (int q = 0; q < 2; ++q) {
+          const int k = kb * 32 + h * 8 + q * 4;
           float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
           if (k < K) v = *reinterpret_cast<const float4*>(A + row * K + k);
           x[4 * q] = v.x; x[4 * q + 1] = v.y; x[4 * q + 2] = v.z; x[4 * q + 3] = v.w;
         }
-        const uint32_t col = A_COL + slot * 64 + h * 16;
-        tc::tmem_st_hilo16(tmem + lane_base + col, tmem + lane_base + col + 32, x);
-      }
-      tc::wait_st();
-      tc::fence_before_sync();
-      tc::mbar_arrive(&a_full[slot]);
-    }
-    tc::mbar_wait(acc_full, 0, err, 2);
-    tc::fence_after_sync();
-#pragma unroll 1
-    for (int c = 0; c < N; c += 16) {
-      float v[16];
-      tc::tmem_ld16(tmem + lane_base + ACC_COL + c, v);
-      tc::wait_ld();
-#pragma unroll
-      for (int q = 0; q < 4; ++q)
-        *reinterpret_cast<float4*>(C + row * N + c + 4 * q) = make_float4(v[4 * q], v[4 * q + 1], v[4 * q + 2], v[4 * q + 3]);
-    }
-    tc::fence_before_sync();
-  } else if (warp == 4) {
-    // ---- B producer: one bulk copy (hi | lo tiles) per k-block ----
-    if (lane == 0) {
-      for (int kb = 0; kb < nkb; ++kb) {
-        const int st = kb % S;
-        tc::mbar_wait(&b_empty[st], ((kb / S) & 1) ^ 1, err, 3);
-        tc::mbar_arrive_expect_tx(&b_full[st], STAGE);
-        tc::bulk_g2s(bst + st * STAGE, reinterpret_cast<const uint8_t*>(Bp) + (size_t)kb * STAGE, STAGE, &b_full[st]);
-      }
-    }
-  } else {
-    // ---- MMA issuer ----
-    if (lane == 0) {
-      constexpr uint32_t idesc = tc::idesc_tf32(128, N);
-      for (int kb = 0; kb < nkb; ++kb) {
-        const int st = kb % S, slot = kb & 1;
-        tc::mbar_wait(&b_full[st], (kb / S) & 1, err, 4);
-        tc::mbar_wait(&a_full[slot], (kb >> 1) & 1, err, 5);
-        tc::fence_after_sync();
-        const int ksteps = min(4, (K - kb * 32) / 8);
-        const uint64_t d_hi = tc::smem_desc_sw128(bst + st * STAGE), d_lo = tc::smem_desc_sw128(bst + st * STAGE + TILE);
-        for (int ks = 0; ks < ksteps; ++ks) {
-          const uint32_t a_hi = tmem + A_COL + slot * 64 + ks * 8, a_lo = a_hi + 32;
-          tc::mma_tf32_ts(tmem + ACC_COL, a_hi, d_hi + 2 * ks, idesc, (kb > 0 || ks > 0) ? 1u : 0u);
-          tc::mma_tf32_ts(tmem + ACC_COL, a_hi, d_lo + 2 * ks, idesc, 1u);
-          tc::mma_tf32_ts(tmem + ACC_COL, a_lo, d_hi + 2 * ks, idesc, 1u);
-        }
-        tc::mma_commit(&a_empty[slot]);
-        tc::mma_commit(&b_empty[st]);
-      }
-      tc::mma_commit(acc_full);
-    }
-  }
-  __syncthreads();
-  if (warp == 5) { tc::fence_after_sync(); tc::tmem_dealloc(tmem, 512); }
-}
-
-// Probe for DESIGN.md 6.1: the same GEMM with the A operand staged in 128B-swizzled SHARED memory (both tcgen05.mma
-// operands from shared-memory descriptors) instead of TMEM -- the form a two-tiles-per-SM cell kernel needs, since
-// it leaves only the 256 accumulator columns of a tile in TMEM.  Not used by the product path.
-template <int N>
-__global__ void __launch_bounds__(192, 1) tc_gemm_ss_test_kernel(const float* __restrict__ A, int K, const float* __restrict__ Bp,
-                                                                 float* __restrict__ C, int* err) {
-  constexpr int S = 2;
-  constexpr uint32_t TILE = N * 128, STAGE = 2 * TILE;
-  constexpr uint32_t A_TILE = 128 * 128, A_SLOT = 2 * A_TILE;          // [hi | lo], 128 rows x 32 floats each
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* bst = smem;
-  uint8_t* ast = smem + S * STAGE;                                      // 2 A slots
-  uint64_t* bars = reinterpret_cast<uint64_t*>(ast + 2 * A_SLOT);
-  uint64_t* b_full = bars, *b_empty = bars + S, *a_full = bars + 2 * S, *a_empty = bars + 2 * S + 2, *acc_full = bars + 2 * S + 4;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * S + 5);
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int nkb = (K + 31) / 32;
-  if (tid == 0) {
-    for (int s = 0; s < S; ++s) { tc::mbar_init(&b_full[s], 1); tc::mbar_init(&b_empty[s], 1); }
-    for (int s = 0; s < 2; ++s) { tc::mbar_init(&a_full[s], 128); tc::mbar_init(&a_empty[s], 1); }
-    tc::mbar_init(acc_full, 1);
-    tc::fence_barrier_init();
-  }
-  if (warp == 5) tc::tmem_alloc(tmem_slot, 256);
-  tc::fence_before_sync();
-  __syncthreads();
-  tc::fence_after_sync();
-  const uint32_t tmem = *tmem_slot;
-
-  if (warp < 4) {
-    const size_t row = (size_t)blockIdx.x * 128 + tid;
-    const uint32_t lane_base = (uint32_t)(warp * 32) << 16;
-    for (int kb = 0; kb < nkb; ++kb) {
-      const int slot = kb & 1;
-      tc::mbar_wait(&a_empty[slot], ((kb >> 1) & 1) ^ 1, err, 1);
-      uint8_t* hi_t = ast + slot * A_SLOT, *lo_t = hi_t + A_TILE;
-#pragma unroll
-      for (int q = 0; q < 8; ++q) {                                       // eight 16-byte chunks of this thread's row
-        const int k = kb * 32 + q * 4;
-        float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (k < K) v = *reinterpret_cast<const float4*>(A + row * K + k);
-        float4 h, l;
-        tc::split_tf32(v.x, h.x, l.x); tc::split_tf32(v.y, h.y, l.y);
-        tc::split_tf32(v.z, h.z, l.z); tc::split_tf32(v.w, h.w, l.w);
-        const uint32_t off = tc::sw128_offset((uint32_t)tid, (uint32_t)(q * 4));
-        *reinterpret_cast<float4*>(hi_t + off) = h;
-        *reinterpret_cast<float4*>(lo_t + off) = l;
+        tc::st_hilo8(hi, hi + A_TILE, (uint32_t)r, (uint32_t)(h * 8), x);
       }
       tc::fence_proxy_async();
-      tc::mbar_arrive(&a_full[slot]);
+      tc::mbar_arrive(&a_full[st]);
     }
-    tc::mbar_wait(acc_full, 0, err, 2);
-    tc::fence_after_sync();
-#pragma unroll 1
-    for (int c = 0; c < N; c += 16) {
-      float v[16];
-      tc::tmem_ld16(tmem + lane_base + c, v);
-      tc::wait_ld();
-#pragma unroll
-      for (int q = 0; q < 4; ++q)
-        *reinterpret_cast<float4*>(C + row * N + c + 4 * q) = make_float4(v[4 * q], v[4 * q + 1], v[4 * q + 2], v[4 * q + 3]);
-    }
-    tc::fence_before_sync();
-  } else if (warp == 4) {
+  } else {
     if (lane == 0) {
       for (int kb = 0; kb < nkb; ++kb) {
         const int st = kb % S;
@@ -218,30 +127,7 @@ __global__ void __launch_bounds__(192, 1) tc_gemm_ss_test_kernel(const float* __
         tc::bulk_g2s(bst + st * STAGE, reinterpret_cast<const uint8_t*>(Bp) + (size_t)kb * STAGE, STAGE, &b_full[st]);
       }
     }
-  } else {
-    if (lane == 0) {
-      constexpr uint32_t idesc = tc::idesc_tf32(128, N);
-      for (int kb = 0; kb < nkb; ++kb) {
-        const int st = kb % S, slot = kb & 1;
-        tc::mbar_wait(&b_full[st], (kb / S) & 1, err, 4);
-        tc::mbar_wait(&a_full[slot], (kb >> 1) & 1, err, 5);
-        tc::fence_after_sync();
-        const int ksteps = min(4, (K - kb * 32) / 8);
-        const uint64_t b_hi = tc::smem_desc_sw128(bst + st * STAGE), b_lo = tc::smem_desc_sw128(bst + st * STAGE + TILE);
-        const uint64_t a_hi = tc::smem_desc_sw128(ast + slot * A_SLOT), a_lo = tc::smem_desc_sw128(ast + slot * A_SLOT + A_TILE);
-        for (int ks = 0; ks < ksteps; ++ks) {
-          tc::mma_tf32_ss(tmem, a_hi + 2 * ks, b_hi + 2 * ks, idesc, (kb > 0 || ks > 0) ? 1u : 0u);
-          tc::mma_tf32_ss(tmem, a_hi + 2 * ks, b_lo + 2 * ks, idesc, 1u);
-          tc::mma_tf32_ss(tmem, a_lo + 2 * ks, b_hi + 2 * ks, idesc, 1u);
-        }
-        tc::mma_commit(&a_empty[slot]);
-        tc::mma_commit(&b_empty[st]);
-      }
-      tc::mma_commit(acc_full);
-    }
   }
-  __syncthreads();
-  if (warp == 5) { tc::fence_after_sync(); tc::tmem_dealloc(tmem, 256); }
 }
 
 }  // namespace
@@ -278,32 +164,13 @@ static int tc_gemm_selftest_impl(const float* A, const float* W, float* C, int M
     pack_b_raw_kernel<<<(total + 255) / 256, 256, 0, st>>>(W, N, K, 0, N, scratch);
     NMARL_LAUNCH_CHECK();
   } else if (nmarl_launch_pack_b(W, N, K, 0, N, scratch, st)) return 1;
-  const size_t smem = 2 * 2 * (size_t)N * 128 + 1024 + 256;
+  const size_t smem = 2 * 2 * (size_t)N * 128 + 2 * 2 * 64 * 128 + 1024 + 256;
   if (N == 256) {
     NMARL_CUDA(cudaFuncSetAttribute(tc_gemm_test_kernel<256>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    tc_gemm_test_kernel<256><<<M / 128, 192, smem, st>>>(A, K, scratch, C, err);
+    tc_gemm_test_kernel<256><<<M / 64, 224, smem, st>>>(A, K, scratch, C, err);
   } else {
     NMARL_CUDA(cudaFuncSetAttribute(tc_gemm_test_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    tc_gemm_test_kernel<64><<<M / 128, 192, smem, st>>>(A, K, scratch, C, err);
-  }
-  NMARL_LAUNCH_CHECK();
-  return 0;
-}
-
-// same GEMM with both operands in shared memory (hardware probe for the two-tiles-per-SM plan; not on the product path)
-extern "C" __attribute__((visibility("default"))) int nmarl_tc_gemm_selftest_ss(const float* A, const float* W, float* C, int M,
-                                                                                  int K, int N, float* scratch, int* err,
-                                                                                  void* stream) {
-  NMARL_CHECK(M > 0 && M % 128 == 0 && K > 0 && K % 8 == 0 && (N == 64 || N == 256), "tc_gemm_selftest_ss: unsupported shape");
-  cudaStream_t st = (cudaStream_t)stream;
-  if (nmarl_launch_pack_b(W, N, K, 0, N, scratch, st)) return 1;
-  const size_t smem = 2 * 2 * (size_t)N * 128 + 2 * 2 * 128 * 128 + 1024 + 256;
-  if (N == 256) {
-    NMARL_CUDA(cudaFuncSetAttribute(tc_gemm_ss_test_kernel<256>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    tc_gemm_ss_test_kernel<256><<<M / 128, 192, smem, st>>>(A, K, scratch, C, err);
-  } else {
-    NMARL_CUDA(cudaFuncSetAttribute(tc_gemm_ss_test_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    tc_gemm_ss_test_kernel<64><<<M / 128, 192, smem, st>>>(A, K, scratch, C, err);
+    tc_gemm_test_kernel<64><<<M / 64, 224, smem, st>>>(A, K, scratch, C, err);
   }
   NMARL_LAUNCH_CHECK();
   return 0;

@@ -1,5 +1,5 @@
-// tc_row.cuh -- shared structure of the tcgen05 cell kernels (forward: tc_cell.cu, backward: tc_bwd.cu):
-// TMEM column map, k-block schedule entries, the row-thread producer helpers and the B-producer / MMA-issuer
+// tc_row.cuh -- shared structure of the tensor-core cell kernels (forward: tc_cell.cu, backward: tc_bwd.cu):
+// shared-memory map, k-block schedule entries, the row-thread producer helpers and the B-producer / MMA-warpgroup
 // role loops.  See tc_cell.cu for the overall design.
 #pragma once
 #include "common.cuh"
@@ -7,23 +7,34 @@
 
 namespace tcrow {
 
-constexpr int S_STAGES = 3;
+constexpr int ROWS = 64;                                 // env rows of a CTA (= wgmma M)
+constexpr int S_STAGES = 2;
 constexpr uint32_t STAGE_BYTES = 2 * 256 * 128;          // hi+lo tiles of the widest operand (N = 256)
-constexpr uint32_t ACC_COL = 0, A_COL = 256;            // TMEM: [0,256) accumulators (encoders reuse it), [256,512) A ring
-// A-operand ring in TMEM: A_SLOTS slots of (hi 32 | lo 32) columns.  4 slots use the whole second half of TMEM; the row
-// threads then run up to four k-blocks ahead of the MMA issuer, which matters for the short encoder GEMMs whose
-// MMAs (N = 64) finish faster than a produce -> commit -> a_empty round trip.
-constexpr int A_SLOTS = 4;
-static_assert((A_SLOTS & (A_SLOTS - 1)) == 0 && A_COL + A_SLOTS * 64 <= 512, "A ring must fit TMEM");
-constexpr int MAX_KB = 40;
+// A-operand ring in shared memory: A_SLOTS slots of [hi | lo] 64-row x 32-deep swizzled tiles
+constexpr int A_SLOTS = 2;
+constexpr uint32_t A_TILE = ROWS * 128, A_SLOT_BYTES = 2 * A_TILE;
+static_assert((A_SLOTS & (A_SLOTS - 1)) == 0, "A ring slots: power of two");
+// accumulator staging: [64 rows][256 columns] fp32; the MMA warpgroup stores finished GEMM results here and the row
+// threads read them back by (row, column).  Columns are XOR-swizzled in 16-byte chunks by (row % 8) so that a warp
+// (32 rows, same column) and the fragment stores both spread over all banks.
+constexpr int ACC_COLS = 256;
+constexpr uint32_t ACC_BYTES = ROWS * ACC_COLS * 4;
+constexpr uint32_t ACC_COL = 0;
+constexpr int MAX_KB = 24;
 // NSET warp-sets share every env row: set s of row r works on columns [s*W, (s+1)*W) of each 32-wide input
-// k-block and on hidden units [s*EW, (s+1)*EW) of the encoders / LSTM cell.  4 sets = 16 row warps per SM
-// (4 per scheduler) so global-load, TMEM and barrier latencies overlap across warps.
+// k-block and on hidden units [s*EW, (s+1)*EW) of the encoders / LSTM cell.
 constexpr int NSET = 4;
 constexpr int W = 32 / NSET, EW = 64 / NSET;
-constexpr int ROW_THREADS = 128 * NSET;
-constexpr int TC_THREADS = ROW_THREADS + 64;
-static_assert(W % 8 == 0 && EW % 8 == 0, "8-column TMEM pieces");
+constexpr int ROW_WARPS = ROWS / 32;                      // warps per set
+constexpr int ROW_THREADS = ROWS * NSET;
+constexpr int MMA_WARP0 = ROW_THREADS / 32;               // warps [MMA_WARP0, +4): the MMA warpgroup
+constexpr int TC_THREADS = ROW_THREADS + 128;
+static_assert(MMA_WARP0 % 4 == 0, "the MMA warps must form an aligned warpgroup");
+static_assert(W == 8 && EW % 8 == 0, "8-column operand pieces");
+
+__device__ __forceinline__ uint32_t acc_idx(uint32_t row, uint32_t col) {
+  return row * ACC_COLS + (col & ~31u) + ((((col >> 2) ^ row) & 7u) << 2) + (col & 3u);
+}
 
 struct KbEnt {
   uint32_t off_bytes, bytes;
@@ -32,7 +43,8 @@ struct KbEnt {
 };
 
 struct RowCtx {
-  uint32_t tmem, lane_base;
+  uint8_t* a_ring; const float* acc;
+  uint32_t r;                                             // env row of this thread inside the CTA
   uint64_t* a_full; uint64_t* a_empty; uint64_t* enc_full;
   int q, e, set;
   int* err;
@@ -41,28 +53,28 @@ struct RowCtx {
 __device__ __forceinline__ void produce_begin(RowCtx& c) {
   const int slot = c.q & (A_SLOTS - 1);
   tc::mbar_wait(&c.a_empty[slot], ((c.q / A_SLOTS) & 1) ^ 1, c.err, 11);
-  tc::fence_after_sync();
 }
 __device__ __forceinline__ void produce_piece(RowCtx& c, int col /*0..31, multiple of 8*/, const float (&x)[8]) {
-  const uint32_t t = c.tmem + c.lane_base + A_COL + (c.q & (A_SLOTS - 1)) * 64 + col;
-  tc::tmem_st_hilo8(t, t + 32, x);
+  uint8_t* hi = c.a_ring + (c.q & (A_SLOTS - 1)) * A_SLOT_BYTES;
+  tc::st_hilo8(hi, hi + A_TILE, c.r, (uint32_t)col, x);
 }
 __device__ __forceinline__ void produce_end(RowCtx& c) {
-  tc::wait_st();
-  tc::fence_before_sync();
+  tc::fence_proxy_async();
   tc::mbar_arrive(&c.a_full[c.q & (A_SLOTS - 1)]);
   c.q++;
+}
+// 8 accumulator columns [col, col + 8) of this thread's row
+__device__ __forceinline__ void acc_ld8(const RowCtx& c, uint32_t col, float (&v)[8]) {
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const float4 t = *reinterpret_cast<const float4*>(c.acc + acc_idx(c.r, col + 4 * h));
+    v[4 * h] = t.x; v[4 * h + 1] = t.y; v[4 * h + 2] = t.z; v[4 * h + 3] = t.w;
+  }
 }
 // one input k-block: this thread contributes columns [set*W, set*W + W)
 __device__ __forceinline__ void produce_in(RowCtx& c, const float (&x)[W]) {
   produce_begin(c);
-#pragma unroll
-  for (int p = 0; p < W / 8; ++p) {
-    float t[8];
-#pragma unroll
-    for (int j = 0; j < 8; ++j) t[j] = x[8 * p + j];
-    produce_piece(c, c.set * W + 8 * p, t);
-  }
+  produce_piece(c, c.set * W, x);
   produce_end(c);
 }
 // two k-blocks fed by a 64-wide activation vector of which this thread holds [set*EW, set*EW + EW)
@@ -87,19 +99,16 @@ __device__ __forceinline__ void produce_act(RowCtx& c, const float (&s)[EW]) {
 __device__ __forceinline__ void enc_wait(RowCtx& c) {
   tc::mbar_wait(c.enc_full, c.e & 1, c.err, 12);
   c.e++;
-  tc::fence_after_sync();
 }
 // this thread's EW columns of a 64-wide result block at accumulator column `col`
 __device__ __forceinline__ void enc_load(RowCtx& c, uint32_t col, float (&v)[EW]) {
 #pragma unroll
   for (int p = 0; p < EW / 8; ++p) {
     float t[8];
-    tc::tmem_ld8(c.tmem + c.lane_base + col + c.set * EW + 8 * p, t);
-    tc::wait_ld();
+    acc_ld8(c, col + c.set * EW + 8 * p, t);
 #pragma unroll
     for (int j = 0; j < 8; ++j) v[8 * p + j] = t[j];
   }
-  tc::fence_before_sync();
 }
 // feature-major saved activations [feature][env]: lane == env row, so one warp access per feature is a single
 // 128-byte line (the row-major form would touch 32 lines per access)
@@ -168,47 +177,62 @@ __device__ __forceinline__ float frcp_(float x) {          // one MUFU.RCP (1 ul
 __device__ __forceinline__ float fsigmoid(float x) { return frcp_(1.0f + __expf(-x)); }
 __device__ __forceinline__ float ftanh(float x) { return fmaf(2.0f, frcp_(1.0f + __expf(-2.0f * x)), -1.0f); }
 __device__ __forceinline__ void row_barrier() { asm volatile("bar.sync 1, %0;" ::"n"(ROW_THREADS) : "memory"); }
+__device__ __forceinline__ void mma_wg_sync() { asm volatile("bar.sync 2, 128;" ::: "memory"); }
 
 
-// ---- role loops (one elected thread each) ------------------------------------------------------------------
-__device__ __forceinline__ void producer_loop(const KbEnt* sched, int n_kb, uint8_t* bst, uint64_t* b_full, uint64_t* b_empty,
-                                              const float* wpack, int* err) {
+// ---- the MMA warpgroup ------------------------------------------------------------------------------------------
+// All 128 threads: per k-block the 3xTF32 wgmma chain into the register accumulator; a finished GEMM (the next entry
+// starts a new one, or a completion flag is set) is stored into the staging area at its column dcol.  Thread 0 also
+// streams the weight k-blocks: one cp.async.bulk (TMA engine) per k-block into the S_STAGES ring, refilled as soon as
+// the warpgroup has retired the MMAs that read a stage.  a_empty / enc_full / acc_full count one arrival per thread.
+__device__ __forceinline__ void mma_loop(const KbEnt* sched, int n_kb, uint8_t* bst, uint8_t* ast, uint64_t* b_full,
+                                         uint64_t* a_full, uint64_t* a_empty, uint64_t* enc_full, uint64_t* acc_full,
+                                         float* acc_s, const float* wpack, int* err) {
+  const int t = threadIdx.x - MMA_WARP0 * 32, w = t >> 5, l = t & 31;
   const uint8_t* wp = reinterpret_cast<const uint8_t*>(wpack);
-  for (int q = 0; q < n_kb; ++q) {
+  auto fetch = [&](int q) {
     const int st = q % S_STAGES;
-    tc::mbar_wait(&b_empty[st], ((q / S_STAGES) & 1) ^ 1, err, 21);
     const KbEnt e = sched[q];
     tc::mbar_arrive_expect_tx(&b_full[st], e.bytes);
     tc::bulk_g2s(bst + st * STAGE_BYTES, wp + e.off_bytes, e.bytes, &b_full[st]);
-  }
-}
-__device__ __forceinline__ void mma_loop(const KbEnt* sched, int n_kb, uint8_t* bst, uint64_t* b_full, uint64_t* b_empty,
-                                         uint64_t* a_full, uint64_t* a_empty, uint64_t* enc_full, uint64_t* acc_full,
-                                         uint32_t tmem, int* err, long long* prof = nullptr) {
+  };
+  if (t == 0)
+    for (int q = 0; q < S_STAGES && q < n_kb; ++q) fetch(q);
+  float d[128];
+#pragma unroll
+  for (int j = 0; j < 128; ++j) d[j] = 0.f;
   for (int q = 0; q < n_kb; ++q) {
     const int st = q % S_STAGES, slot = q & (A_SLOTS - 1);
     const KbEnt e = sched[q];
     tc::mbar_wait(&b_full[st], (q / S_STAGES) & 1, err, 31);
-    if (prof) prof[32 + 3 * q] = clock64();
     tc::mbar_wait(&a_full[slot], (q / A_SLOTS) & 1, err, 32);
-    tc::fence_after_sync();
-    if (prof) prof[33 + 3 * q] = clock64();
-    const uint32_t tile = e.bytes / 2;
-    const uint32_t ncols = tile / 128;                       // N of this operand
-    const uint64_t d_hi = tc::smem_desc_sw128(bst + st * STAGE_BYTES), d_lo = tc::smem_desc_sw128(bst + st * STAGE_BYTES + tile);
-    const uint32_t idesc = tc::idesc_tf32(128, ncols);
-    const uint32_t dcol = tmem + e.dcol;
-    for (int ks = 0; ks < e.ksteps; ++ks) {
-      const uint32_t a_hi = tmem + A_COL + slot * 64 + ks * 8, a_lo = a_hi + 32;
-      tc::mma_tf32_ts(dcol, a_hi, d_hi + 2 * ks, idesc, (e.first && ks == 0) ? 0u : 1u);
-      tc::mma_tf32_ts(dcol, a_hi, d_lo + 2 * ks, idesc, 1u);
-      tc::mma_tf32_ts(dcol, a_lo, d_hi + 2 * ks, idesc, 1u);
+    const int N = (int)(e.bytes / 256);
+    uint8_t* b = bst + st * STAGE_BYTES;
+    uint8_t* a = ast + slot * A_SLOT_BYTES;
+    tc::wgmma_fence();
+    tc::wgmma_kblock_3x(N, d, tc::smem_desc_sw128(a), tc::smem_desc_sw128(a + A_TILE), tc::smem_desc_sw128(b),
+                        tc::smem_desc_sw128(b + N * 128), e.ksteps, e.first != 0);
+    tc::wgmma_commit();
+    tc::wgmma_wait_all();
+    tc::mbar_arrive(&a_empty[slot]);
+    mma_wg_sync();                                         // every thread has retired the k-block: stage st is free
+    if (t == 0 && q + S_STAGES < n_kb) fetch(q + S_STAGES);
+    if (e.last_enc || e.last_acc || q + 1 == n_kb || sched[q + 1].first) {
+      const uint32_t r0 = 16 * w + (l >> 2);
+#pragma unroll
+      for (int j = 0; j < 32; ++j) {
+        if (8 * j < N) {
+          const uint32_t col = e.dcol + 8 * j + 2 * (l & 3);
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const uint32_t r = r0 + 8 * h;
+            *reinterpret_cast<float2*>(acc_s + acc_idx(r, col)) = make_float2(d[4 * j + 2 * h], d[4 * j + 2 * h + 1]);
+          }
+        }
+      }
+      if (e.last_enc) tc::mbar_arrive(enc_full);
+      if (e.last_acc) tc::mbar_arrive(acc_full);
     }
-    tc::mma_commit(&a_empty[slot]);
-    tc::mma_commit(&b_empty[st]);
-    if (e.last_enc) tc::mma_commit(enc_full);
-    if (e.last_acc) tc::mma_commit(acc_full);
-    if (prof) prof[34 + 3 * q] = clock64();
   }
 }
 __device__ __forceinline__ KbEnt make_kb(int off_floats, int N, int K, int kb, int dcol, int first, int last_enc, int last_acc) {
@@ -221,6 +245,34 @@ __device__ __forceinline__ KbEnt make_kb(int off_floats, int N, int K, int kb, i
   e.pad0 = e.pad1 = 0;
   return e;
 }
-constexpr size_t TC_SMEM = S_STAGES * STAGE_BYTES + 1024 /*align slack*/ + 32 * 8 /*mbarriers*/ + 16 + MAX_KB * sizeof(KbEnt) + NSET * 128 * 8 * sizeof(float);
+// [B stages | A slots | accumulator staging | mbarriers | schedule], 1024-byte aligned tiles
+struct Smem {
+  uint8_t* bst; uint8_t* ast; float* acc;
+  uint64_t *b_full, *a_full, *a_empty, *enc_full, *acc_full;
+  int* n_kb; KbEnt* sched;
+};
+__device__ __forceinline__ Smem smem_map(uint8_t* raw) {
+  uint8_t* s = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(raw) + 1023) & ~uintptr_t(1023));
+  Smem m;
+  m.bst = s;
+  m.ast = s + S_STAGES * STAGE_BYTES;
+  m.acc = reinterpret_cast<float*>(m.ast + A_SLOTS * A_SLOT_BYTES);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(m.acc) + ACC_BYTES);
+  m.b_full = bars; m.a_full = bars + S_STAGES; m.a_empty = m.a_full + A_SLOTS;
+  m.enc_full = m.a_empty + A_SLOTS; m.acc_full = m.enc_full + 1;
+  m.n_kb = reinterpret_cast<int*>(m.acc_full + 1);
+  m.sched = reinterpret_cast<KbEnt*>(m.n_kb + 2);
+  return m;
+}
+__device__ __forceinline__ void init_barriers(const Smem& s) {
+  for (int i = 0; i < S_STAGES; ++i) tc::mbar_init(&s.b_full[i], 1);
+  for (int i = 0; i < A_SLOTS; ++i) { tc::mbar_init(&s.a_full[i], ROW_THREADS); tc::mbar_init(&s.a_empty[i], 128); }
+  tc::mbar_init(s.enc_full, 128);
+  tc::mbar_init(s.acc_full, 128);
+  tc::fence_barrier_init();
+}
+constexpr size_t TC_SMEM = 1024 /*align slack*/ + S_STAGES * STAGE_BYTES + A_SLOTS * A_SLOT_BYTES + ACC_BYTES + 16 * 8 /*mbarriers*/ +
+                           8 + MAX_KB * sizeof(KbEnt);
+static_assert(TC_SMEM <= 232448, "cell kernels exceed the 227 KB of dynamic shared memory");
 
 }  // namespace tcrow

@@ -1,9 +1,10 @@
-// tc_wgrad.cu -- tcgen05 weight gradients of every GEMM of the cell (gate matrix and the obs / fingerprint /
-// message encoders):   dW[ka][n] = sum over all (t, env) rows r of  A[r][ka] * D[r][n]
-// as 3xTF32 GEMMs with M = ka (one 128-lane tile per job), the contraction over rows split across CTAs and a
-// fixed-order reduce afterwards.
-//   A operand: the saved activations are feature-major ([t][agent][feature][env]); TMEM lane = feature ka, so
-//              a thread reads 8 consecutive envs (32 contiguous bytes), splits hi/lo and tcgen05.st's them.
+// tc_wgrad.cu -- tensor-core (wgmma) weight gradients of every GEMM of the cell (gate matrix and the obs /
+// fingerprint / message encoders):   dW[ka][n] = sum over all (t, env) rows r of  A[r][ka] * D[r][n]
+// as 3xTF32 GEMMs with M = ka (each 128-lane job is two 64-lane CTAs), the contraction over rows split across CTAs
+// and a fixed-order reduce afterwards.
+//   A operand: the saved activations are feature-major ([t][agent][feature][env]); operand row = feature ka, so
+//              a thread reads 8 consecutive envs (32 contiguous bytes), splits hi/lo and stores them into the
+//              swizzled shared-memory ring.
 //   B operand: D^T, K-major over rows, was written by the backward cell kernel as ready-made [hi | lo]
 //              128B-swizzled tiles (dz: 256 rows, encoder pre-activation grads: 192/128/64 rows); the producer
 //              bulk-copies the needed row range of the tile per 32 env rows.
@@ -18,17 +19,15 @@ namespace {
 using namespace tcrow;
 
 enum { J_GATE0 = 0, J_GATE1, J_ENC_X, J_ENC_M0, J_ENC_M1, J_COUNT };
-// Row-thread roles: warp-sets 0,1 produce the A operand (16 of the 32 columns of a k-block each), warp-sets 2,3 derive
-// the `lo` half of the raw B tiles in shared memory; the two dependent chains (global load -> split -> tcgen05.st
-// and TMA wait -> lds/sts -> proxy fence) run side by side instead of back to back in every thread.
-constexpr int A_SETS = 2, A_THREADS = 128 * A_SETS, WA = 32 / A_SETS;
-// Shared-memory rings.  RAW tiles: WG_RAW_STAGES single 32 KB raw tiles (bulk-copied, deep enough to cover the DRAM
-// latency of a 32 KB copy at one k-block per ~0.8 us) + WG_LO_BUFS derived `lo` tiles; [hi | lo] pairs: S_STAGES x 64 KB.
-constexpr int WG_RAW_STAGES = 5, WG_LO_BUFS = 2;
-constexpr uint32_t WG_RAW_BYTES = 256 * 128;
-constexpr size_t WG_SMEM_RAW = (size_t)(WG_RAW_STAGES + WG_LO_BUFS) * WG_RAW_BYTES + 1024 + 32 * 8 + 64;
-static_assert(WG_SMEM_RAW <= 232448, "wgrad RAW ring exceeds the 227 KB of dynamic shared memory");
-constexpr int SEG_KB = 20;       // k-blocks (of 32 rows) accumulated in TMEM before the accumulator is drained (see flush)
+// Row threads: 4 sets x 64 feature lanes; set s produces envs [8s, 8s + 8) of every 32-env k-block.
+constexpr int WG_LANES = 64, WG_SETS = 4, WA = 32 / WG_SETS;
+constexpr int WG_A_THREADS = WG_LANES * WG_SETS;
+constexpr int WG_MMA_WARP0 = WG_A_THREADS / 32, WG_THREADS = WG_A_THREADS + 128;
+constexpr int WG_STAGES = 3;
+constexpr size_t WG_SMEM = 1024 + (size_t)WG_STAGES * STAGE_BYTES + A_SLOTS * A_SLOT_BYTES + 16 * 8;
+static_assert(WG_SMEM <= 232448, "wgrad rings exceed the 227 KB of dynamic shared memory");
+static_assert(WG_LANES == ROWS, "A tiles of the wgrad kernel have the cell kernels' 64 rows");
+constexpr int SEG_KB = 20;       // k-blocks (of 32 rows) accumulated in registers before the accumulator is drained
 
 struct TcWgK {
   int B, T, splits, ndp;
@@ -38,7 +37,6 @@ struct TcWgK {
   long long ws_off[J_COUNT];     // float offset of each job's partial block [splits][N_agents][128][N_job]
   int jobs[J_COUNT]; int n_jobs; // job kinds present
   int* err;
-  long long* prof;               // debug: clock64 stamps of CTA (split 1, job 0, agent 1) or NULL (tools/wg_prof.py)
 };
 
 struct JobDesc {
@@ -69,31 +67,24 @@ __device__ __forceinline__ JobDesc job_desc(const nmarl_model& m, const TcWgK& k
   return d;
 }
 
-// RAW (experimental, DESIGN.md 6.2): the D^T tiles hold raw fp32 once.  The producer copies one tile per k-block; it
-// doubles as the hi operand (the TF32 datapath drops the 13 low mantissa bits -- tools/probe_tf32_operand.py); the
-// row threads derive lo = x - trunc(x) into the second half of the stage and signal lo_full; the issuer runs the two
-// passes that need only the raw tile first and a_hi * b_lo after that barrier.
+// RAW: the D^T tiles hold raw fp32 once.  One tile per k-block is copied into the hi half of the stage; the MMA
+// warpgroup splits it in place into the same rounded [hi | lo] pair the packed tiles carry (tc::split_tf32) before
+// the k-block's MMAs.
 template <bool RAW>
-__global__ void __launch_bounds__(TC_THREADS, 1) tc_wgrad_kernel(const __grid_constant__ nmarl_model m,
+__global__ void __launch_bounds__(WG_THREADS, 1) tc_wgrad_kernel(const __grid_constant__ nmarl_model m,
                                                                  const __grid_constant__ TcWgK k) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* bst = smem;
-  constexpr int NST = RAW ? WG_RAW_STAGES : S_STAGES;                  // B stages
-  constexpr uint32_t STB = RAW ? WG_RAW_BYTES : STAGE_BYTES;           // bytes per B stage
-  uint8_t* lobuf = smem + (size_t)NST * STB;                           // RAW only: WG_LO_BUFS derived lo tiles
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + (size_t)NST * STB + (RAW ? WG_LO_BUFS * WG_RAW_BYTES : 0));
-  uint64_t* b_full = bars, *b_empty = bars + NST, *a_full = bars + 2 * NST, *a_empty = a_full + A_SLOTS;
-  uint64_t* enc_full = a_empty + A_SLOTS, *acc_full = enc_full + 1;
-  uint64_t* acc_free = acc_full + 1;                                   // accumulator drained by the row threads (segment flush)
-  uint64_t* lo_full = acc_free + 1, *lo_empty = lo_full + WG_LO_BUFS;  // RAW only
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(lo_empty + WG_LO_BUFS);
+  uint8_t* ast = smem + (size_t)WG_STAGES * STAGE_BYTES;
+  uint64_t* bars = reinterpret_cast<uint64_t*>(ast + A_SLOTS * A_SLOT_BYTES);
+  uint64_t* b_full = bars, *a_full = bars + WG_STAGES, *a_empty = a_full + A_SLOTS;
 
-  const int sp = blockIdx.x, jslot = blockIdx.y, i = blockIdx.z;
+  const int sp = blockIdx.x, jslot = blockIdx.y >> 1, mh = blockIdx.y & 1, i = blockIdx.z;
   const int kind = k.jobs[jslot];
   const JobDesc d = job_desc(m, k, kind, i);
   const int N_agents = m.n_agent;
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int tid = threadIdx.x, warp = tid >> 5;
   const int bpt = k.B / 32;                                           // 32-row k-blocks per time step
   const int kb_total = k.T * bpt;
   const int per = (kb_total + k.splits - 1) / k.splits;
@@ -102,20 +93,11 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_wgrad_kernel(const __grid_co
   float* wsj = k.ws + k.ws_off[jslot] + ((size_t)sp * N_agents + i) * 128 * d.N;
 
   if (tid == 0) {
-    for (int s = 0; s < NST; ++s) { tc::mbar_init(&b_full[s], 1); tc::mbar_init(&b_empty[s], 1); }
-    for (int s = 0; s < A_SLOTS; ++s) { tc::mbar_init(&a_full[s], A_THREADS); tc::mbar_init(&a_empty[s], 1); }
-    tc::mbar_init(enc_full, 1);
-    tc::mbar_init(acc_full, 1);
-    tc::mbar_init(acc_free, ROW_THREADS);
-    if constexpr (RAW)
-      for (int s = 0; s < WG_LO_BUFS; ++s) { tc::mbar_init(&lo_full[s], ROW_THREADS - A_THREADS); tc::mbar_init(&lo_empty[s], 1); }
+    for (int s = 0; s < WG_STAGES; ++s) tc::mbar_init(&b_full[s], 1);
+    for (int s = 0; s < A_SLOTS; ++s) { tc::mbar_init(&a_full[s], WG_A_THREADS); tc::mbar_init(&a_empty[s], 128); }
     tc::fence_barrier_init();
   }
-  if (warp == ROW_THREADS / 32 + 1) tc::tmem_alloc(tmem_slot, 512);
-  tc::fence_before_sync();
   __syncthreads();
-  tc::fence_after_sync();
-  const uint32_t tmem = *tmem_slot;
   const uint32_t tile_bytes = (uint32_t)d.N * 128u;                   // hi (or lo) part staged per k-block
   // byte offset of the D^T tile of (t, 32-env block rb): [hi | lo] pairs, or single raw tiles packed inside each
   // time step's (unchanged) [hi | lo]-sized slab
@@ -126,12 +108,10 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_wgrad_kernel(const __grid_co
     return reinterpret_cast<const uint8_t*>(d.BT) + off;
   };
 
-  if (warp < ROW_THREADS / 32) {
-    RowCtx c;
-    const int set = warp >> 2, quarter = warp & 3;
-    const int ka = quarter * 32 + lane;                               // TMEM lane == feature within this M tile
-    c.tmem = tmem; c.lane_base = (uint32_t)(quarter * 32) << 16;
-    c.a_full = a_full; c.a_empty = a_empty; c.enc_full = enc_full; c.q = 0; c.e = 0; c.set = set; c.err = k.err;
+  if (warp < WG_MMA_WARP0) {
+    // ---- A producers: feature lane `row` of this CTA, envs [set * WA, set * WA + WA) of every k-block ----------------
+    const int row = tid % WG_LANES, set = tid / WG_LANES;
+    const int ka = mh * WG_LANES + row;                               // feature within the job's 128-lane tile
     const bool one = d.ones && ka == d.ka_cnt;
     const bool is_p = ka > d.ka_cnt && ka <= d.ka_cnt + d.p_cnt;
     const bool real = ka < d.ka_cnt || is_p;
@@ -147,8 +127,8 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_wgrad_kernel(const __grid_co
         hs_agent = m.agent[i].nbr[fm / NH]; hs_unit = fm % NH;
       }
     }
-    // the A operand of k-block q: 8 consecutive envs of this thread's feature (global loads; issued one k-block AHEAD so
-    // that their latency hides behind the lo pass / the barrier waits of the current k-block)
+    // the A operand of k-block q: 8 consecutive envs of this thread's feature (global loads; issued two k-blocks AHEAD
+    // so that their latency hides behind the barrier waits of the current k-block)
     auto load_x = [&](int q, float (&x)[WA]) {
       const int kb = kb0 + q, t = kb / bpt, rb = kb - t * bpt;
       if (hs_agent >= 0) {
@@ -178,158 +158,90 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_wgrad_kernel(const __grid_co
         for (int j = 0; j < WA; ++j) x[j] = one ? 1.0f : 0.0f;
       }
     };
-    // Segmented accumulation.  The tensor core adds every MMA into the fp32 accumulator with round-toward-zero: a bias
-    // of ~2^-24 of the running sum per MMA that grows linearly with the chain length (measured 1.4e-4 of max|g| after
-    // the 2 496 MMAs of one B = 4096, T = 60 split).  The accumulator is therefore drained every SEG_KB k-blocks
-    // (240 MMAs at SEG_KB = 20) and the segment sums are added up in the CTA's own workspace slot with ordinary
-    // round-to-nearest fp32 adds.
-    const bool warp_active = quarter * 32 < d.ka_cnt + (d.ones ? 1 : 0) + d.p_cnt;   // tcgen05.ld is warp-collective
-    float* out = wsj + ka;                                      // element (ka, n) of the partial block at out[n * 128]
-    // The previous partial sums are fetched BEFORE the wait for the segment's last MMAs (the loads do not depend on
-    // them) in two batches of four 8-column pieces, so that one L2 round trip, not eight, is exposed per drain.
-    long long* prof = (k.prof != nullptr && sp == 1 && jslot == 0 && i == 1 && (tid == 0 || tid == A_THREADS)) ? k.prof + (tid ? 128 : 192) : nullptr;
-    auto flush = [&](int seg) {
-      if (prof && seg < 5) prof[3 * seg] = clock64();
-      const bool mine = warp_active && (real || one);
-      const bool rmw = mine && seg > 0;
-      tc::mbar_wait(acc_full, seg & 1, k.err, 13);
-      tc::fence_after_sync();
-      if (prof && seg < 5) prof[3 * seg + 1] = clock64();
-      // workspace block layout [column n][lane ka]: for a fixed column the 32 lanes of a warp are 128 contiguous bytes
-#pragma unroll 2
-      for (int c0 = set * 8; c0 < d.N; c0 += 8 * NSET) {
-        if (warp_active) {                                         // warp-uniform: tcgen05.ld is warp-collective
-          float pv[8];
-          if (rmw) {
-#pragma unroll
-            for (int j = 0; j < 8; ++j) pv[j] = out[(size_t)(c0 + j) * 128];
-          }
-          float v[8];
-          tc::tmem_ld8(tmem + c.lane_base + ACC_COL + c0, v);
-          tc::wait_ld();
-          if (mine) {
-#pragma unroll
-            for (int j = 0; j < 8; ++j) out[(size_t)(c0 + j) * 128] = rmw ? v[j] + pv[j] : v[j];
-          }
-        }
-      }
-      tc::fence_before_sync();
-      if (prof && seg < 5) prof[3 * seg + 2] = clock64();
-      tc::mbar_arrive(acc_free);
+    float xa[WA], xb[WA];                     // the operands of the next two k-blocks (two loads in flight per thread)
+    auto emit_a = [&](int q, float (&x)[WA]) {
+      const int slot = q & (A_SLOTS - 1);
+      tc::mbar_wait(&a_empty[slot], ((q / A_SLOTS) & 1) ^ 1, k.err, 11);
+      uint8_t* hi = ast + slot * A_SLOT_BYTES;
+      tc::st_hilo8(hi, hi + A_TILE, (uint32_t)row, (uint32_t)(set * WA), x);
+      tc::fence_proxy_async();
+      tc::mbar_arrive(&a_full[slot]);
+      if (q + 2 < nkb) load_x(q + 2, x);        // refill this buffer; it is consumed two k-blocks from now
     };
-    if (set < A_SETS) {
-      // ---- A producers: columns [set * WA, set * WA + WA) of every k-block, loads issued one k-block ahead ------------
-      float xa[WA], xb[WA];                     // the operands of the next two k-blocks (two loads in flight per thread)
-      auto emit_a = [&](int q, float (&x)[WA]) {
-        produce_begin(c);
-#pragma unroll
-        for (int p = 0; p < WA / 8; ++p) {
-          float t8[8];
-#pragma unroll
-          for (int j = 0; j < 8; ++j) t8[j] = x[8 * p + j];
-          produce_piece(c, set * WA + 8 * p, t8);
-        }
-        produce_end(c);
-        if (q + 2 < nkb) load_x(q + 2, x);        // refill this buffer; it is consumed two k-blocks from now
-        if ((q + 1) % SEG_KB == 0 || q + 1 == nkb) flush(q / SEG_KB);
-      };
-      if (nkb > 0) load_x(0, xa);
-      if (nkb > 1) load_x(1, xb);
-      for (int q = 0; q < nkb; q += 2) {
-        emit_a(q, xa);
-        if (q + 1 < nkb) emit_a(q + 1, xb);
-      }
-    } else {
-      // ---- lo derivation (RAW tiles): lo = rn_tf32(x - trunc_tf32(x)) of the k-block's B stage ---------------------------
-      const int lt = tid - A_THREADS;
-      for (int q = 0; q < nkb; ++q) {
-        if constexpr (RAW) {
-          const int st = q % NST, lb = q % WG_LO_BUFS;
-          tc::mbar_wait(&lo_empty[lb], ((q / WG_LO_BUFS) & 1) ^ 1, k.err, 42);      // the MMAs that read this lo buffer are done
-          tc::mbar_wait(&b_full[st], (q / NST) & 1, k.err, 41);
-          const float4* raw = reinterpret_cast<const float4*>(bst + (size_t)st * STB);
-          float4* lo = reinterpret_cast<float4*>(lobuf + (size_t)lb * WG_RAW_BYTES);
-          for (uint32_t e = (uint32_t)lt; e < tile_bytes / 16; e += ROW_THREADS - A_THREADS) {
-            const float4 v = raw[e];
-            float4 l;
-            l.x = tc::tf32_lo_of_raw(v.x); l.y = tc::tf32_lo_of_raw(v.y);
-            l.z = tc::tf32_lo_of_raw(v.z); l.w = tc::tf32_lo_of_raw(v.w);
-            lo[e] = l;
-          }
-          tc::fence_proxy_async();
-          tc::mbar_arrive(&lo_full[lb]);
-        }
-        if ((q + 1) % SEG_KB == 0 || q + 1 == nkb) flush(q / SEG_KB);
-      }
-    }
-    if (nkb == 0 && warp_active && (real || one)) {
-      for (int c0 = set * 8; c0 < d.N; c0 += 8 * NSET)
-        for (int j = 0; j < 8; ++j) out[(size_t)(c0 + j) * 128] = 0.f;
-    }
-  } else if (warp == ROW_THREADS / 32) {
-    if (tc::elect_one()) {
-      for (int q = 0; q < nkb; ++q) {
-        const int kb = kb0 + q, st = q % NST;
-        const int t = kb / bpt, rb = kb - t * bpt;
-        tc::mbar_wait(&b_empty[st], ((q / NST) & 1) ^ 1, k.err, 21);
-        const uint8_t* tile = bt_tile(t, rb);
-        if constexpr (RAW) {
-          tc::mbar_arrive_expect_tx(&b_full[st], tile_bytes);
-          tc::bulk_g2s(bst + (size_t)st * STB, tile + (size_t)d.n_row0 * 128, tile_bytes, &b_full[st]);
-        } else {
-          tc::mbar_arrive_expect_tx(&b_full[st], 2 * tile_bytes);
-          tc::bulk_g2s(bst + (size_t)st * STB, tile + (size_t)d.n_row0 * 128, tile_bytes, &b_full[st]);
-          tc::bulk_g2s(bst + (size_t)st * STB + tile_bytes, tile + (size_t)(d.tile_rows + d.n_row0) * 128, tile_bytes, &b_full[st]);
-        }
-      }
+    if (nkb > 0) load_x(0, xa);
+    if (nkb > 1) load_x(1, xb);
+    for (int q = 0; q < nkb; q += 2) {
+      emit_a(q, xa);
+      if (q + 1 < nkb) emit_a(q + 1, xb);
     }
   } else {
-    if (tc::elect_one()) {
-      const uint32_t idesc = tc::idesc_tf32(128, (uint32_t)d.N);
-      long long* iprof = (k.prof != nullptr && sp == 1 && jslot == 0 && i == 1) ? k.prof : nullptr;
-      for (int q = 0; q < nkb; ++q) {
-        const int st = q % NST, slot = q & (A_SLOTS - 1), lb = q % WG_LO_BUFS;
-        if (iprof && q < 40) iprof[3 * q] = clock64();
-        const int seg = q / SEG_KB;
-        const bool seg_first = (q % SEG_KB) == 0;
-        if (seg_first && seg > 0) tc::mbar_wait(acc_free, (seg - 1) & 1, k.err, 34);   // previous segment drained
-        tc::mbar_wait(&b_full[st], (q / NST) & 1, k.err, 31);
-        tc::mbar_wait(&a_full[slot], (q / A_SLOTS) & 1, k.err, 32);
-        tc::fence_after_sync();
-        const uint64_t d_hi = tc::smem_desc_sw128(bst + (size_t)st * STB);
-        const uint64_t d_lo = tc::smem_desc_sw128(RAW ? lobuf + (size_t)lb * WG_RAW_BYTES : bst + (size_t)st * STB + tile_bytes);
-        if constexpr (RAW) {
+    // ---- MMA warpgroup; its thread 0 also bulk-copies the D^T tiles into the WG_STAGES ring --------------------------
+    // Segmented accumulation: the accumulator is drained into the CTA's workspace slot every SEG_KB k-blocks
+    // (240 MMAs) and the segment sums are added up there with ordinary round-to-nearest fp32 adds, which bounds the
+    // error growth of a single long accumulation chain.
+    const int t = tid - WG_MMA_WARP0 * 32, w = t >> 5, l = t & 31;
+    // workspace block layout [column n][lane ka]
+    float* out = wsj + mh * WG_LANES + 16 * w + (l >> 2);
+    auto fetch = [&](int q) {
+      const int kb = kb0 + q, st = q % WG_STAGES;
+      const int tt = kb / bpt, rb = kb - tt * bpt;
+      const uint8_t* tile = bt_tile(tt, rb);
+      tc::mbar_arrive_expect_tx(&b_full[st], RAW ? tile_bytes : 2 * tile_bytes);
+      tc::bulk_g2s(bst + (size_t)st * STAGE_BYTES, tile + (size_t)d.n_row0 * 128, tile_bytes, &b_full[st]);
+      if (!RAW)
+        tc::bulk_g2s(bst + (size_t)st * STAGE_BYTES + tile_bytes, tile + (size_t)(d.tile_rows + d.n_row0) * 128, tile_bytes, &b_full[st]);
+    };
+    if (t == 0)
+      for (int q = 0; q < WG_STAGES && q < nkb; ++q) fetch(q);
+    float acc[128];
 #pragma unroll
-          for (int ks = 0; ks < 4; ++ks) {                              // passes that need only the raw tile
-            const uint32_t a_hi = tmem + A_COL + slot * 64 + ks * 8, a_lo = a_hi + 32;
-            tc::mma_tf32_ts(tmem + ACC_COL, a_hi, d_hi + 2 * ks, idesc, (seg_first && ks == 0) ? 0u : 1u);
-            tc::mma_tf32_ts(tmem + ACC_COL, a_lo, d_hi + 2 * ks, idesc, 1u);
-          }
-          if (iprof && q < 40) iprof[3 * q + 1] = clock64();
-          tc::mbar_wait(&lo_full[lb], (q / WG_LO_BUFS) & 1, k.err, 33);
-          tc::fence_after_sync();
-          if (iprof && q < 40) iprof[3 * q + 2] = clock64();
+    for (int j = 0; j < 128; ++j) acc[j] = 0.f;
+    auto drain = [&](bool rmw) {
 #pragma unroll
-          for (int ks = 0; ks < 4; ++ks)
-            tc::mma_tf32_ts(tmem + ACC_COL, tmem + A_COL + slot * 64 + ks * 8, d_lo + 2 * ks, idesc, 1u);
-        } else {
+      for (int j = 0; j < 32; ++j) {
+        if (8 * j < d.N) {
+          const int n = 8 * j + 2 * (l & 3);
 #pragma unroll
-          for (int ks = 0; ks < 4; ++ks) {
-            const uint32_t a_hi = tmem + A_COL + slot * 64 + ks * 8, a_lo = a_hi + 32;
-            tc::mma_tf32_ts(tmem + ACC_COL, a_hi, d_hi + 2 * ks, idesc, (seg_first && ks == 0) ? 0u : 1u);
-            tc::mma_tf32_ts(tmem + ACC_COL, a_hi, d_lo + 2 * ks, idesc, 1u);
-            tc::mma_tf32_ts(tmem + ACC_COL, a_lo, d_hi + 2 * ks, idesc, 1u);
+          for (int e = 0; e < 4; ++e) {
+            float* o = out + (size_t)(n + (e & 1)) * 128 + 8 * (e >> 1);
+            *o = rmw ? *o + acc[4 * j + e] : acc[4 * j + e];
           }
         }
-        tc::mma_commit(&a_empty[slot]);
-        tc::mma_commit(&b_empty[st]);
-        if constexpr (RAW) tc::mma_commit(&lo_empty[lb]);
-        if ((q + 1) % SEG_KB == 0 || q + 1 == nkb) tc::mma_commit(acc_full);
       }
+    };
+    for (int q = 0; q < nkb; ++q) {
+      const int st = q % WG_STAGES, slot = q & (A_SLOTS - 1);
+      const bool seg_first = (q % SEG_KB) == 0;
+      uint8_t* b = bst + (size_t)st * STAGE_BYTES;
+      tc::mbar_wait(&b_full[st], (q / WG_STAGES) & 1, k.err, 31);
+      if constexpr (RAW) {
+        float4* hi = reinterpret_cast<float4*>(b);
+        float4* lo = reinterpret_cast<float4*>(b + tile_bytes);
+        for (uint32_t e = (uint32_t)t; e < tile_bytes / 16; e += 128) {
+          const float4 v = hi[e];
+          float4 h, lo4;
+          tc::split_tf32(v.x, h.x, lo4.x); tc::split_tf32(v.y, h.y, lo4.y);
+          tc::split_tf32(v.z, h.z, lo4.z); tc::split_tf32(v.w, h.w, lo4.w);
+          hi[e] = h;
+          lo[e] = lo4;
+        }
+        tc::fence_proxy_async();
+        mma_wg_sync();
+      }
+      tc::mbar_wait(&a_full[slot], (q / A_SLOTS) & 1, k.err, 32);
+      uint8_t* a = ast + slot * A_SLOT_BYTES;
+      tc::wgmma_fence();
+      tc::wgmma_kblock_3x(d.N, acc, tc::smem_desc_sw128(a), tc::smem_desc_sw128(a + A_TILE), tc::smem_desc_sw128(b),
+                          tc::smem_desc_sw128(b + tile_bytes), 4, seg_first);
+      tc::wgmma_commit();
+      tc::wgmma_wait_all();
+      tc::mbar_arrive(&a_empty[slot]);
+      mma_wg_sync();                              // every thread has retired the k-block: stage st is free
+      if (t == 0 && q + WG_STAGES < nkb) fetch(q + WG_STAGES);
+      if ((q + 1) % SEG_KB == 0 || q + 1 == nkb) drain(q >= SEG_KB);
     }
+    if (nkb == 0) drain(false);                // acc is zero: the reduce reads every lane of the block
   }
-  __syncthreads();
-  if (warp == ROW_THREADS / 32 + 1) { tc::fence_after_sync(); tc::tmem_dealloc(tmem, 512); }
 }
 
 // fixed-order reduce over the row splits + scatter into the flat gradient buffer
@@ -357,7 +269,7 @@ __global__ void __launch_bounds__(256) tc_wgrad_reduce_kernel(const __grid_const
 }
 
 // gate bias gradient: fixed-order reduce of the per-tile partial sums the backward cell kernel left in sv_dz
-// ([t][agent][tile][256]); one CTA per (32 columns, agent), 8 strided partial chains per column + an ordered tail
+// ([t][agent][32-row tile][256]); one CTA per (32 columns, agent), 8 strided partial chains per column + an ordered tail
 __global__ void __launch_bounds__(256) gate_bias_reduce_kernel(const __grid_constant__ nmarl_model m, const float* __restrict__ part,
                                                               int tiles, int T, float* __restrict__ grads) {
   __shared__ float red[8][32];
@@ -400,8 +312,8 @@ int job_N(const nmarl_model* m, int kind) {
 int nmarl_tc_ndp(const nmarl_model* m) { return m->variant == NMARL_NC ? 192 : (m->variant == NMARL_IA2C ? 64 : 128); }
 
 int nmarl_tc_wgrad_splits(int n_agent) {
-  int s = 37;                                   // 2 gate tiles x 37 x 8 agents = 592 CTAs = 4 waves of 148 SMs
-  while (2 * s * n_agent > 148 * 8 && s > 1) s = (s + 1) / 2;
+  int s = 33;                                   // 2 gate tiles x 2 halves x 33 x 8 agents = 1056 CTAs = 8 waves of 132 SMs
+  while (4 * s * n_agent > 132 * 8 && s > 1) s = (s + 1) / 2;
   return s;
 }
 
@@ -420,21 +332,22 @@ int nmarl_tc_launch_wgrads(const nmarl_model* m, int B, int T, const float* sv_s
   k.B = B; k.T = T; k.splits = nmarl_tc_wgrad_splits(m->n_agent); k.ndp = nmarl_tc_ndp(m);
   k.sv_sh = sv_sh; k.sv_xin = sv_xin; k.dzT = dzT; k.dpT = dpT; k.ws = ws; k.err = err;
   k.h_seq = h_seq; k.done_pre = done_pre;
-  k.prof = g_nmarl_prof;
   k.n_jobs = job_list(m, k.jobs);
   long long off = 0;
   for (int j = 0; j < k.n_jobs; ++j) { k.ws_off[j] = off; off += (long long)k.splits * m->n_agent * 128 * job_N(m, k.jobs[j]); }
   static bool configured = false;
   if (!configured) {
-    NMARL_CUDA(cudaFuncSetAttribute(tc_wgrad_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TC_SMEM));
-    NMARL_CUDA(cudaFuncSetAttribute(tc_wgrad_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)WG_SMEM_RAW));
+    NMARL_CUDA(cudaFuncSetAttribute(tc_wgrad_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)WG_SMEM));
+    NMARL_CUDA(cudaFuncSetAttribute(tc_wgrad_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)WG_SMEM));
     configured = true;
   }
-  gate_bias_reduce_kernel<<<dim3(NG / 32, m->n_agent), 256, 0, st_bias>>>(*m, sv_dz, B / 128, T, grads);   // independent of the GEMM jobs
+  // independent of the GEMM jobs; the backward cell kernel leaves one partial per 32 env rows
+  gate_bias_reduce_kernel<<<dim3(NG / 32, m->n_agent), 256, 0, st_bias>>>(*m, sv_dz, B / 32, T, grads);
   NMARL_LAUNCH_CHECK();
   if (ev_wgrad) NMARL_CUDA(cudaEventRecord((cudaEvent_t)ev_wgrad[0], st));
-  if (raw_tiles) tc_wgrad_kernel<true><<<dim3(k.splits, k.n_jobs, m->n_agent), TC_THREADS, WG_SMEM_RAW, st>>>(*m, k);
-  else tc_wgrad_kernel<false><<<dim3(k.splits, k.n_jobs, m->n_agent), TC_THREADS, TC_SMEM, st>>>(*m, k);
+  const dim3 grid(k.splits, 2 * k.n_jobs, m->n_agent);               // y: (job, 64-lane half of its 128-lane tile)
+  if (raw_tiles) tc_wgrad_kernel<true><<<grid, WG_THREADS, WG_SMEM, st>>>(*m, k);
+  else tc_wgrad_kernel<false><<<grid, WG_THREADS, WG_SMEM, st>>>(*m, k);
   NMARL_LAUNCH_CHECK();
   if (ev_wgrad) NMARL_CUDA(cudaEventRecord((cudaEvent_t)ev_wgrad[1], st));
   NMARL_DBG_SYNC(st, "tc_wgrad_kernel");

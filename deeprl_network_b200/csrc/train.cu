@@ -978,8 +978,8 @@ extern "C" int nmarl_a2c_bptt(const nmarl_model* m, const nmarl_bwd_args* a, voi
     k.wpack = a->wpack; k.tc_err = a->tc_err; k.state_fm = a->state_fm;
     k.raw_tiles = raw_tiles;
     const bool use_tc = (a->wpack != nullptr && B % 128 == 0 && m->kx_pad <= 32 && m->kp_pad <= 32);
-    // tensor-core path: sv_dz holds the per-tile gate-bias partial sums [T][N][B/128][256]; FFMA path: dz [T][N][B][256]
-    k.sv_dz = use_tc ? a->sv_dz + (size_t)t * N * (B / 128) * NG : a->sv_dz + (size_t)t * nb * NG;
+    // tensor-core path: sv_dz holds the gate-bias partial sums of every 32 env rows [T][N][B/32][256]; FFMA path: dz [T][N][B][256]
+    k.sv_dz = use_tc ? a->sv_dz + (size_t)t * N * (B / 32) * NG : a->sv_dz + (size_t)t * nb * NG;
     k.dzT = (use_tc && a->sv_dzT) ? a->sv_dzT + (size_t)t * N * (B / 32) * (2 * 256 * 32) : nullptr;
     k.ndp = nmarl_tc_ndp(m);
     k.dpT = (use_tc && a->sv_dpT) ? a->sv_dpT + (size_t)t * N * (B / 32) * (2 * k.ndp * 32) : nullptr;

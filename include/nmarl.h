@@ -1,4 +1,4 @@
-/* nmarl.h -- C ABI of the B200-native networked-MARL hot path (libnmarl.so).
+/* nmarl.h -- C ABI of the H100-native networked-MARL hot path (libnmarl.so).
  *
  * Drop-in boundary (SURVEY.md 8b): the reference has no FFI; the surface it exposes is the
  * Python env/agent API.  This header is what the Python mirror of that API
@@ -12,7 +12,7 @@
  * inside an opaque `nmarl_ctx`: one helper stream + two events used to fork side work beside the
  * BPTT chain, created by nmarl_create and freed by nmarl_destroy; entry points that fork take
  * the ctx through their argument block.  Re-entrant per ctx, not thread-safe per ctx.  All launches
- * are asynchronous on the given stream and are CUDA-graph capturable.  Device code is sm_100a only.
+ * are asynchronous on the given stream and are CUDA-graph capturable.  Device code is sm_90a only.
  *
  * Layout: every per-agent tensor is agent-major, env-minor: X[agent][env][feature]
  * (so an agent's rows are contiguous for its grouped GEMM, and the env kernel is coalesced
@@ -144,7 +144,7 @@ typedef struct {
   const int32_t* act_in;   /* v-call / train: [N][B] same-step actions                         */
   float* v;                /* v-call: [N][B]                                                   */
   const float* wpack;      /* packed 3xTF32 operands (nmarl_pack_weights) or NULL.  When set and  */
-                           /* B % 128 == 0 the tcgen05 tensor-core kernel is used, else FP32 FFMA */
+                           /* B % 128 == 0 the wgmma tensor-core kernel is used, else FP32 FFMA */
   int32_t* tc_err;         /* device int: tensor-core pipeline watchdog (0 = ok); may be NULL      */
   /* optional (p-call, tensor-core path only): save the activations BPTT needs while rolling out, so the
    * update can skip the separate training forward (same inputs, same weights => same numbers):         */
@@ -154,7 +154,7 @@ typedef struct {
 
 int nmarl_policy_step_p(const nmarl_model* m, const nmarl_fwd_args* a, void* stream);
 int nmarl_policy_step_v(const nmarl_model* m, const nmarl_fwd_args* a, void* stream);
-/* Pack the GEMM weights for the tcgen05 path: per 32-wide k-block a [hi | lo] pair of 128B-swizzled
+/* Pack the GEMM weights for the tensor-core path: per 32-wide k-block a [hi | lo] pair of 128B-swizzled
  * K-major tiles of W^T (hi = value rounded to TF32, lo = rounded remainder).  Call after every parameter
  * change.  wt (transposed weights scratch, n_wt floats) is also refreshed.                           */
 int nmarl_pack_weights(const nmarl_model* m, const float* params, float* wt, float* wpack, void* stream);
@@ -188,7 +188,7 @@ int nmarl_nstep_return_adv(int n_agent, int B, int T, int NR, const double* rewa
  *   sv_xin [T][N][B][kx_pad+kp_pad+km_pad]  sv_sh [T][N][B][s_dim+64]  sv_gates [T][N][B][256]
  *   sv_enc [T][N][B][128] (IC3: 64 used; DIAL: 128)   sv_dlv [T][N][B][8]
  *   sv_dz [T][N][B][256]   sv_dpre [T][N][B][192]   sv_dmp [T][N][B][64] (DIAL)
- *   (tensor-core path: sv_dz = [T][N][B/128][256] per-tile gate-bias partial sums, sv_dpre unused)
+ *   (tensor-core path: sv_dz = [T][N][B/32][256] gate-bias partial sums per 32 rows, sv_dpre unused)
  *   dh_rec, dc_rec [2][N][B][64]   dmsg [2][N][MAX_NBR][B][64]
  *   wt [n_wt] transposed weights   ws: split-K workspace of ws_floats floats
  *   loss_part float [T][N][tiles][4] per-CTA partial sums (policy, value, entropy, pad)

@@ -1,4 +1,4 @@
-"""Command line of the B200-native CACC / networked-A2C hot path.
+"""Command line of the H100-native CACC / networked-A2C hot path.
 
 The reference's command line is kept verbatim (main.py:21-40 there) so existing scripts keep working:
 

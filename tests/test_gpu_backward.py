@@ -41,7 +41,7 @@ def _oracle_backward(orc, lay, batch, lr=5e-4, apply=False, hp=HP):
 
 
 @pytest.mark.parametrize('variant', VARIANTS)
-@pytest.mark.parametrize('T,B', [(6, 1), (5, 37), (3, 130), (3, 128), (4, 256)])    # B % 128 == 0: tcgen05 forward + backward
+@pytest.mark.parametrize('T,B', [(6, 1), (5, 37), (3, 130), (3, 128), (4, 256)])    # B % 128 == 0: tensor-core forward + backward
 def test_gradients_match_oracle_autograd(variant, T, B):
     eng, orc, lay, params = make_pair(variant, B, T=T, dtype=torch.float64)
     batch = _batch(eng, lay, T, B)

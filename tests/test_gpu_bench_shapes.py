@@ -1,4 +1,4 @@
-"""GPU: parity of the tcgen05 (tensor-core) path AT THE SHAPES bench.py TIMES (VERDICT r1, item 1).
+"""GPU: parity of the tensor-core path AT THE SHAPES bench.py TIMES (VERDICT r1, item 1).
 
 For each BASELINE.json configuration, at its per-GPU batch:
   cfg2  config_ma2c_nc_catchup.ini      NeurComm, 8 agents, B = 4096, T = 60   (the headline shape)

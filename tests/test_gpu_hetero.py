@@ -3,7 +3,7 @@
     tests/golden/hetero_*.npz -- recorded from the UNMODIFIED reference MA2C_NC / MA2C_IC3 / MA2C_DIAL classes with
     n_s = [5,7,4,6,5,3], n_a = [4,3,5,2,4,3] on the TF shim -- and must reproduce every pi / v / R within 1e-5 and the
     weights after three updates within 2e-5, starting from the same NumPy-stream initial weights (exact).
-(2) The batched kernels (FFMA and tcgen05 paths) against the batched oracle: pi / v / state 1e-5, gradients
+(2) The batched kernels (FFMA and tensor-core paths) against the batched oracle: pi / v / state 1e-5, gradients
     2e-5 x scale against float64 autograd, and the zero-padding of the embedding receives exactly zero gradient."""
 import hashlib
 
@@ -71,7 +71,7 @@ def _inputs(rs, shape, n_s, n_a):
 
 
 @pytest.mark.parametrize('agent', AGENTS)
-@pytest.mark.parametrize('B', [7, 128])                     # 128: tcgen05 path
+@pytest.mark.parametrize('B', [7, 128])                     # 128: tensor-core path
 def test_hetero_kernels_match_oracle(agent, B):
     T = 4
     eng, orc, lay, n_s, n_a = _pair(agent, B, T)

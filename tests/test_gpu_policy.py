@@ -24,7 +24,7 @@ def _inputs(B, N=8, seed=0):
 
 
 @pytest.mark.parametrize('variant', VARIANTS)
-@pytest.mark.parametrize('B', [1, 37, 130, 128, 256])       # 128/256 take the tcgen05 path
+@pytest.mark.parametrize('B', [1, 37, 130, 128, 256])       # 128/256 take the tensor-core path
 def test_p_and_v_calls_match_oracle(variant, B):
     from deeprl_network_b200 import _lib as L
     eng, orc, lay, _ = make_pair(variant, B)

@@ -1,5 +1,5 @@
-"""GPU: the tcgen05 (5th-gen tensor core) building blocks.  3xTF32 split GEMM with the A operand in
-TMEM, B in 128B-swizzled shared memory via bulk copies, FP32 accumulation in TMEM, against float64."""
+"""GPU: the wgmma tensor-core building blocks.  3xTF32 split GEMM with both operands in 128B-swizzled shared
+memory (B via bulk copies), FP32 accumulation in registers, against float64."""
 import ctypes as C
 
 import numpy as np
@@ -37,7 +37,7 @@ def test_3xtf32_gemm_matches_fp64(M, K, N):
 
 @pytest.mark.parametrize('variant', ['ma2c_nc', 'ma2c_ic3', 'ma2c_dial', 'ia2c'])
 def test_tensor_core_cell_matches_ffma_cell(variant):
-    """The tcgen05 forward (B % 128 == 0) and the FP32-FFMA forward are two implementations of the same
+    """The tensor-core forward (B % 128 == 0) and the FP32-FFMA forward are two implementations of the same
     step: identical pi / v / state to ~1e-6, identical sampled actions, DIAL messages included."""
     import sys, os
     sys.path.insert(0, os.path.dirname(__file__))

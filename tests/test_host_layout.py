@@ -131,12 +131,10 @@ def test_no_product_import_of_oracle():
 
 def test_shipped_configs_equal_the_reference_configs():
     """Drop-in contract: every CACC .ini of the reference runs unchanged (key- and value-identical copies under
-    config/).  Needs the reference checkout, which exists only in the build container."""
+    config/).  tests/golden/reference_config holds verbatim copies of the reference repository's CACC configs."""
     import configparser
     import glob
-    ref_dir = '/root/reference/config'
-    if not os.path.isdir(ref_dir):
-        pytest.skip('reference checkout not present')
+    ref_dir = os.path.join(ROOT, 'tests', 'golden', 'reference_config')
     names = sorted(os.path.basename(f) for f in glob.glob(os.path.join(ref_dir, 'config_*_catchup.ini')) +
                    glob.glob(os.path.join(ref_dir, 'config_*_slowdown.ini')))
     assert len(names) == 12
