@@ -30,11 +30,6 @@ __device__ __forceinline__ void split_tf32(float x, float& hi, float& lo) {
   split_tf32(x, h, l);
   hi = __uint_as_float(h); lo = __uint_as_float(l);
 }
-// remainder of a RAW fp32 operand the tensor core reads truncated (it ignores the 13 low mantissa bits)
-__device__ __forceinline__ float tf32_lo_of_raw(float x) {
-  return __uint_as_float(tf32_rn(x - __uint_as_float(__float_as_uint(x) & 0xFFFFE000u)));
-}
-
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
 // ---- programmatic dependent launch (PDL) --------------------------------------------------------------------

@@ -10,8 +10,9 @@
 namespace {
 using namespace tcrow;
 
-// RAW (experimental, DESIGN.md 6.2): the operand tiles for the weight-gradient GEMMs are stored once as raw fp32
-// instead of as a [hi | lo] pair; the weight-gradient kernel derives lo in shared memory.
+// RAW (the default; nmarl_bwd_args.raw_tiles): the operand tiles for the weight-gradient GEMMs are stored once as raw
+// fp32 instead of as a [hi | lo] pair; the weight-gradient kernel splits them in shared memory with the same
+// tc::split_tf32, so both forms feed its MMAs identical operands.
 template <int VAR, bool FM, bool RAW>
 __global__ void __launch_bounds__(TC_THREADS, 1) tc_cell_bwd_kernel(const __grid_constant__ nmarl_model m,
                                                                     const __grid_constant__ BwdK k) {

@@ -158,10 +158,12 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_cell_fwd_kernel(const __grid
     STAMP();
     // ---- encoder GEMMs: A chunks back to back, one completion wait ----------------------------------------------
     const int xm0 = m.kx_pad + m.kp_pad;
-    if (SAVE && c0 < m.kx_pad) st_fm<W>(xin_fm, c0, B, b, xv);
+    // kx_pad / kp_pad are multiples of 4, the column slices 8 wide: e.g. the 25 IA2C inputs on the 5x5 grid pad to 28,
+    // and features 28..31 of the last slice would land on the next section (or the next agent's row of sv_xin)
+    if (SAVE && c0 < m.kx_pad) st_fm<W>(xin_fm, c0, B, b, xv, m.kx_pad - c0);
     produce_in(c, xv);
     if (VAR == NMARL_NC) {
-      if (SAVE && c0 < m.kp_pad) st_fm<W>(xin_fm, m.kx_pad + c0, B, b, pv);
+      if (SAVE && c0 < m.kp_pad) st_fm<W>(xin_fm, m.kx_pad + c0, B, b, pv, m.kp_pad - c0);
       produce_in(c, pv);
     }
     if (VAR == NMARL_IC3) {

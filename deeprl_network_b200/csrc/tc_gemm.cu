@@ -1,6 +1,6 @@
 // tc_gemm.cu -- weight packing for the tensor-core path + a stand-alone 3xTF32 GEMM used by the tests to
 // validate the tensor-core pipeline (swizzled operand tiles, wgmma descriptors, bulk copies, mbarriers)
-// in isolation:  C[M x N] = A[M x K] * W[K x N]   (M % 128 == 0, K % 8 == 0, N in {64, 256}).
+// in isolation:  C[M x N] = A[M x K] * W[K x N]   (M % 128 == 0, K % 8 == 0, N in {64, 128, 192, 256}).
 #include "common.cuh"
 #include "tc.cuh"
 
@@ -23,24 +23,6 @@ __global__ void pack_b_kernel(const float* __restrict__ W, int ldw, int K, int n
     const uint32_t off = tc::sw128_offset(n, kk);
     *reinterpret_cast<float*>(tile + off) = hi;
     *reinterpret_cast<float*>(tile + (size_t)nrows * 128 + off) = lo;
-  }
-}
-
-// Probe variant of the packing (tools/probe_tf32_operand.py): the "hi" tile holds the RAW fp32 values, the "lo" tile
-// x - trunc_tf32(x) as before.  If the TF32 datapath ignores the 13 low mantissa bits of a shared-memory operand,
-// a GEMM on these tiles is bit-identical to one on the masked tiles, and operand tiles written by the backward
-// kernel would not need a separate hi copy (DESIGN.md 6.2).
-__global__ void pack_b_raw_kernel(const float* __restrict__ W, int ldw, int K, int n0, int nrows, float* __restrict__ out) {
-  const int nkb = (K + 31) / 32;
-  const int total = nkb * nrows * 32;
-  for (int idx = blockIdx.x * blockDim.x + threadIdx.x; idx < total; idx += gridDim.x * blockDim.x) {
-    const int n = idx % nrows, kk = (idx / nrows) % 32, kb = idx / (nrows * 32);
-    const int k = kb * 32 + kk;
-    const float x = (k < K) ? W[(size_t)k * ldw + n0 + n] : 0.f;
-    char* tile = reinterpret_cast<char*>(out) + (size_t)kb * 2 * nrows * 128;
-    const uint32_t off = tc::sw128_offset(n, kk);
-    *reinterpret_cast<float*>(tile + off) = x;
-    *reinterpret_cast<float*>(tile + (size_t)nrows * 128 + off) = tc::tf32_lo_of_raw(x);
   }
 }
 
@@ -139,39 +121,24 @@ int nmarl_launch_pack_b(const float* W, int ldw, int K, int n0, int nrows, float
   return 0;
 }
 
-static int tc_gemm_selftest_impl(const float* A, const float* W, float* C, int M, int K, int N, float* scratch, int* err,
-                                 void* stream, bool raw_hi);
-
 // C[M x N] = A[M x K] * W[K x N]; scratch must hold ceil(K/32) * 2 * N * 32 floats; err: device int (0 = ok)
 extern "C" __attribute__((visibility("default"))) int nmarl_tc_gemm_selftest(const float* A, const float* W, float* C, int M, int K,
                                                                                int N, float* scratch, int* err, void* stream) {
-  return tc_gemm_selftest_impl(A, W, C, M, K, N, scratch, err, stream, false);
-}
-
-// same GEMM with the un-masked operand in the hi tile (hardware probe, not used by the product path)
-extern "C" __attribute__((visibility("default"))) int nmarl_tc_gemm_selftest_raw(const float* A, const float* W, float* C, int M,
-                                                                                   int K, int N, float* scratch, int* err,
-                                                                                   void* stream) {
-  return tc_gemm_selftest_impl(A, W, C, M, K, N, scratch, err, stream, true);
-}
-
-static int tc_gemm_selftest_impl(const float* A, const float* W, float* C, int M, int K, int N, float* scratch, int* err,
-                                 void* stream, bool raw_hi) {
-  NMARL_CHECK(M > 0 && M % 128 == 0 && K > 0 && K % 8 == 0 && (N == 64 || N == 256), "tc_gemm_selftest: unsupported shape");
+  NMARL_CHECK(M > 0 && M % 128 == 0 && K > 0 && K % 8 == 0 && (N == 64 || N == 128 || N == 192 || N == 256),
+              "tc_gemm_selftest: unsupported shape");
   cudaStream_t st = (cudaStream_t)stream;
-  if (raw_hi) {
-    const int total = ((K + 31) / 32) * N * 32;
-    pack_b_raw_kernel<<<(total + 255) / 256, 256, 0, st>>>(W, N, K, 0, N, scratch);
-    NMARL_LAUNCH_CHECK();
-  } else if (nmarl_launch_pack_b(W, N, K, 0, N, scratch, st)) return 1;
+  if (nmarl_launch_pack_b(W, N, K, 0, N, scratch, st)) return 1;
   const size_t smem = 2 * 2 * (size_t)N * 128 + 2 * 2 * 64 * 128 + 1024 + 256;
-  if (N == 256) {
-    NMARL_CUDA(cudaFuncSetAttribute(tc_gemm_test_kernel<256>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    tc_gemm_test_kernel<256><<<M / 64, 224, smem, st>>>(A, K, scratch, C, err);
-  } else {
-    NMARL_CUDA(cudaFuncSetAttribute(tc_gemm_test_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    tc_gemm_test_kernel<64><<<M / 64, 224, smem, st>>>(A, K, scratch, C, err);
+  auto run = [&](auto kern) -> int {
+    NMARL_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    kern<<<M / 64, 224, smem, st>>>(A, K, scratch, C, err);
+    NMARL_LAUNCH_CHECK();
+    return 0;
+  };
+  switch (N) {     // one wgmma shape per width: m64n64k8, m64n128k8, m64n192k8, m64n256k8
+    case 64: return run(tc_gemm_test_kernel<64>);
+    case 128: return run(tc_gemm_test_kernel<128>);
+    case 192: return run(tc_gemm_test_kernel<192>);
+    default: return run(tc_gemm_test_kernel<256>);
   }
-  NMARL_LAUNCH_CHECK();
-  return 0;
 }

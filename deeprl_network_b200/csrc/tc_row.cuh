@@ -113,11 +113,13 @@ __device__ __forceinline__ void enc_load(RowCtx& c, uint32_t col, float (&v)[EW]
 // feature-major saved activations [feature][env]: lane == env row, so one warp access per feature is a single
 // 128-byte line (the row-major form would touch 32 lines per access)
 template <int NV>
-__device__ __forceinline__ void st_fm(float* base, int f0, int B, int b, const float (&v)[NV]) {
+__device__ __forceinline__ void st_fm(float* base, int f0, int B, int b, const float (&v)[NV], int n = NV) {
   // saved activations are written once and read once much later (BPTT): streaming stores keep them from
-  // evicting the weights and the recurrent state the next calls re-read from L2
+  // evicting the weights and the recurrent state the next calls re-read from L2.  Only the first n features are
+  // stored: a section narrower than the thread's column slice must not spill into the next one.
 #pragma unroll
-  for (int j = 0; j < NV; ++j) __stcs(base + (size_t)(f0 + j) * B + b, v[j]);
+  for (int j = 0; j < NV; ++j)
+    if (j < n) __stcs(base + (size_t)(f0 + j) * B + b, v[j]);
 }
 template <int NV>
 __device__ __forceinline__ void ld_fm(const float* base, int f0, int B, int b, float (&v)[NV]) {

@@ -53,3 +53,20 @@ def obs_dev(lay, base):
     o = np.zeros((N, B, lay.obs_stride), dtype=np.float32)
     o[:, :, :5] = np.swapaxes(base, 0, 1)
     return to_dev(o)
+
+
+class ScriptedEnv:
+    """Device stand-in for CACCEnv in `PolicyEngine.rollout`: step t writes the pre-generated observations and dones of
+    slot t + 1 (and zero rewards), whatever actions were sampled.  Lets the fused rollout path (rollout p-calls that
+    save the BPTT activations, then `backward`) run on any layout -- heterogeneous ones included -- and any done
+    pattern.  obs: device [T+1, N, B, obs_stride]; done: device [T+1, B] (slot t = done before step t)."""
+
+    def __init__(self, obs, done):
+        self.obs, self.done, self.t = obs, done, 0
+
+    def step_device(self, action, obs_out=None, reward_out=None, greward_out=None, done_out=None):
+        self.t += 1
+        obs_out.copy_(self.obs[self.t])
+        done_out.copy_(self.done[self.t])
+        reward_out.zero_()
+        greward_out.zero_()

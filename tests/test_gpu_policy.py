@@ -58,9 +58,18 @@ def test_p_and_v_calls_match_oracle(variant, B):
 
 @pytest.mark.parametrize('variant', VARIANTS)
 def test_greedy_actions_bit_exact(variant):
+    _greedy_actions_bit_exact(variant, 200)
+
+
+@pytest.mark.parametrize('variant', VARIANTS)
+def test_greedy_actions_bit_exact_tensor_core(variant):
+    _greedy_actions_bit_exact(variant, 256)         # whole 128-env tiles: the tensor-core forward samples greedily
+
+
+def _greedy_actions_bit_exact(variant, B):
     from deeprl_network_b200 import _lib as L
-    B = 200
     eng, orc, lay, _ = make_pair(variant, B, scale=1.0)
+    assert eng.use_tc == (B % 128 == 0)
     rs, base, fp, done, c0, h0 = _inputs(B, seed=3)
     eng.set_states(nb(c0), nb(h0))
     orc.states_fw = torch.tensor(np.concatenate([c0, h0], -1))

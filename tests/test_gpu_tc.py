@@ -9,7 +9,12 @@ import torch
 pytestmark = pytest.mark.gpu
 
 
-@pytest.mark.parametrize('M,K,N', [(128, 32, 256), (256, 256, 256), (128, 8, 64), (128, 16, 64), (384, 128, 64), (128, 72, 256)])
+# every wgmma width the kernels use (m64n64k8 ... m64n256k8), K from one 8-deep k-step to several 32-deep k-blocks,
+# with K % 32 != 0 (a partial last k-block) at every width
+@pytest.mark.parametrize('M,K,N', [(128, 32, 256), (256, 256, 256), (128, 8, 64), (128, 16, 64), (384, 128, 64), (128, 72, 256),
+                                   (128, 8, 128), (256, 40, 128), (128, 256, 128), (384, 104, 128),
+                                   (128, 8, 192), (256, 56, 192), (128, 256, 192), (384, 136, 192),
+                                   (256, 200, 64), (256, 24, 256)])
 def test_3xtf32_gemm_matches_fp64(M, K, N):
     from deeprl_network_b200 import _lib as L
     lib = L.lib()

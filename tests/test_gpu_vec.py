@@ -96,13 +96,25 @@ def test_batched_rollout_and_update_vs_oracle(agent):
 
 
 def test_graph_replay_equals_eager():
+    _graph_replay_equals_eager('ma2c_nc', 16)
+
+
+@pytest.mark.parametrize('agent', ['ma2c_nc', 'ma2c_ic3', 'ma2c_dial', 'ia2c', 'ia2c_fp', 'ma2c_cu'])
+def test_graph_replay_equals_eager_tensor_core(agent):
+    """B = 128: the captured graph replays the tensor-core update (saved rollout + fused BPTT) that bench.py times."""
+    _graph_replay_equals_eager(agent, 128)
+
+
+def _graph_replay_equals_eager(agent, B):
     outs = []
     for graph in (False, True):
-        cp, env, model, vt = _make('ma2c_nc', 16, graph=graph)
+        cp, env, model, vt = _make(agent, B, graph=graph)
+        assert model.engine.use_tc == (B % 128 == 0)
         vt.start()
         for _ in range(3):
             vt.update()
         torch.cuda.synchronize()
+        model.engine.check_tc()
         outs.append((model.engine.params.clone(), model.engine.grew_buf.clone(), env.t_dev.clone()))
     assert torch.equal(outs[0][0], outs[1][0]) and torch.equal(outs[0][1], outs[1][1]) and torch.equal(outs[0][2], outs[1][2])
 
