@@ -162,7 +162,9 @@ __global__ void __launch_bounds__(16 * TY) cell_fwd_kernel(const __grid_constant
     for (int q = 0; q < TM; ++q) { acc[q][0] = acc[q][1] = acc[q][2] = acc[q][3] = 0.f; }
     const int Km = (VAR == NMARL_IC3) ? NH : ag.n_nbr * NH;
     gemm_rowA<TM, 1, TY, KC>(acc, IN + MO, LDI, Km, P + ag.o_w_msg, NH, WsE, tid);
-    const float4 bb = *reinterpret_cast<const float4*>(P + ag.o_b_msg + 4 * tx);
+    // DIAL without a message encoder (o_b_msg < 0, see nmarl.h): relu(0 + 0) = 0 and no own-action one-hot below
+    const bool has_msg = ag.o_b_msg >= 0;
+    const float4 bb = has_msg ? *reinterpret_cast<const float4*>(P + ag.o_b_msg + 4 * tx) : make_float4(0.f, 0.f, 0.f, 0.f);
 #pragma unroll
     for (int q = 0; q < TM; ++q) {
       const int r = ty + TY * q;
@@ -175,8 +177,8 @@ __global__ void __launch_bounds__(16 * TY) cell_fwd_kernel(const __grid_constant
             make_float4(sv[q][0] + z[0], sv[q][1] + z[1], sv[q][2] + z[2], sv[q][3] + z[3]);
       } else {                                                          // DIAL: relu + relu + onehot(argmax p_i)
         float hm[4] = {fmaxf(z[0], 0.f), fmaxf(z[1], 0.f), fmaxf(z[2], 0.f), fmaxf(z[3], 0.f)};
-        int am = 0;
-        if (r < rows) {
+        int am = has_msg ? 0 : -1;
+        if (r < rows && has_msg) {
           const float* pr = a.fp + ((size_t)i * B + b0 + r) * n_a;
           float best = pr[0];
           for (int c = 1; c < n_a; ++c) { const float pv = pr[c]; if (pv > best) { best = pv; am = c; } }
@@ -440,6 +442,8 @@ int check_model(const nmarl_model* m) {
     NMARL_CHECK(m->variant != NMARL_IC3 || m->km_pad >= NH, "CommNet needs km_pad >= 64");
     NMARL_CHECK(m->variant != NMARL_NC || ag.n_nbr * m->n_a <= m->kp_pad, "agent %d: fingerprint width exceeds kp_pad", i);
     NMARL_CHECK(m->variant != NMARL_IC3 || ag.n_nbr > 0, "agent %d: CommNet needs >= 1 neighbour", i);
+    NMARL_CHECK(m->variant == NMARL_IA2C || ag.o_b_msg >= 0 || (m->variant == NMARL_DIAL && ag.n_nbr == 0),
+                "agent %d: only a DIAL agent without neighbours may lack the message encoder", i);
   }
   return 0;
 }

@@ -49,16 +49,19 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_cell_fwd_kernel(const __grid
     init_barriers(sm);
     // ---- k-block schedule shared by the three roles: all encoder GEMMs first (each into its own 64-column
     // block of the accumulator region, one completion barrier), then the gate GEMM over [s | h^] ----------------
+    // An agent without neighbours has zero-width fingerprint / message operands: they get no k-block (and no packed
+    // tiles to copy), and the row threads feed relu(0 + b) for them, as the FFMA kernel does.
     int n = 0;
     const int KG = SD + NH, nG = KG / 32;
-    sched[n++] = make_kb(ag.tp_x, 64, Kx, 0, ACC_COL, 1, VAR == NMARL_IA2C, 0);          // X (Kx <= 32 on this path)
-    if (VAR == NMARL_NC) sched[n++] = make_kb(ag.tp_p, 64, ag.n_nbr * n_a, 0, ACC_COL + 64, 1, 0, 0);
+    sched[n++] = make_kb(ag.tp_x, 64, Kx, 0, ACC_COL, 1, 0, 0);                          // X (Kx <= 32 on this path)
+    if (VAR == NMARL_NC && ag.n_nbr > 0) sched[n++] = make_kb(ag.tp_p, 64, ag.n_nbr * n_a, 0, ACC_COL + 64, 1, 0, 0);
     if (VAR != NMARL_IA2C) {
       const int nM = (VAR == NMARL_IC3) ? 2 : 2 * ag.n_nbr;
       const int KM = (VAR == NMARL_IC3) ? NH : NH * ag.n_nbr;
       const int mcol = (VAR == NMARL_NC) ? ACC_COL + 128 : ACC_COL + 64;
-      for (int j = 0; j < nM; ++j) sched[n++] = make_kb(ag.tp_m, 64, KM, j, mcol, j == 0, j == nM - 1, 0);
+      for (int j = 0; j < nM; ++j) sched[n++] = make_kb(ag.tp_m, 64, KM, j, mcol, j == 0, 0, 0);
     }
+    sched[n - 1].last_enc = 1;                          // the last encoder GEMM actually scheduled completes enc_full
     for (int g = 0; g < nG; ++g) sched[n++] = make_kb(ag.tp_g, 256, KG, g, ACC_COL, g == 0, 0, g == nG - 1);
     if (VAR == NMARL_DIAL && MODE != MODE_V)
       for (int j = 0; j < 2; ++j) sched[n++] = make_kb(ag.tp_mfc, 64, NH, j, ACC_COL, j == 0, j == 1, 0);
@@ -164,7 +167,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_cell_fwd_kernel(const __grid
     produce_in(c, xv);
     if (VAR == NMARL_NC) {
       if (SAVE && c0 < m.kp_pad) st_fm<W>(xin_fm, m.kx_pad + c0, B, b, pv, m.kp_pad - c0);
-      produce_in(c, pv);
+      if (ag.n_nbr > 0) produce_in(c, pv);              // no fingerprint k-block without neighbours (schedule above)
     }
     if (VAR == NMARL_IC3) {
 #pragma unroll
@@ -205,10 +208,16 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_cell_fwd_kernel(const __grid
     enc_load(c, ACC_COL, s0);
     bias_act(s0, P + ag.o_b_ob + e0, VAR == NMARL_IC3 ? 1 : 0);
     if (SAVE && (VAR == NMARL_IC3 || VAR == NMARL_DIAL)) st_fm<EW>(enc_fm, e0, B, b, s0);
+    // an encoder GEMM that was not scheduled (no neighbours) contributes 0 before its bias
+    auto enc_load_or_0 = [&](bool present, uint32_t col, float (&v)[EW]) {
+      if (present) { enc_load(c, col, v); return; }
+#pragma unroll
+      for (int j = 0; j < EW; ++j) v[j] = 0.f;
+    };
     if (VAR == NMARL_NC) {
       float s1[EW], s2[EW];
-      enc_load(c, ACC_COL + 64, s1);
-      enc_load(c, ACC_COL + 128, s2);
+      enc_load_or_0(ag.n_nbr > 0, ACC_COL + 64, s1);
+      enc_load_or_0(ag.n_nbr > 0, ACC_COL + 128, s2);
       bias_act(s1, P + ag.o_b_fp + e0, 0);
       bias_act(s2, P + ag.o_b_msg + e0, 0);
       if (SAVE) { st_fm<EW>(sh_fm, e0, B, b, s0); st_fm<EW>(sh_fm, NH + e0, B, b, s1); st_fm<EW>(sh_fm, 2 * NH + e0, B, b, s2); }
@@ -220,16 +229,18 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_cell_fwd_kernel(const __grid
       produce_act(c, s0);
     } else {
       float s1[EW];
-      enc_load(c, ACC_COL + 64, s1);
+      enc_load_or_0(VAR == NMARL_IC3 || ag.n_nbr > 0, ACC_COL + 64, s1);
       if (VAR == NMARL_IC3) {                                            // s = tanh(..) + m W_msg + b  (utils.py:400)
         bias_act(s1, P + ag.o_b_msg + e0, 2);
 #pragma unroll
         for (int j = 0; j < EW; ++j) s0[j] += s1[j];
       } else {                                                           // DIAL: relu + relu + onehot(argmax p_i)
-        bias_act(s1, P + ag.o_b_msg + e0, 0);
+        // without a message encoder (o_b_msg < 0, see nmarl.h) s is the observation encoder alone: s1 stays 0, no one-hot
+        const bool has_msg = ag.o_b_msg >= 0;
+        if (has_msg) bias_act(s1, P + ag.o_b_msg + e0, 0);
         if (SAVE) st_fm<EW>(enc_fm, NH + e0, B, b, s1);
-        int am = 0;
-        {
+        int am = has_msg ? 0 : -1;
+        if (has_msg) {
           const float* pr = a.fp + row * n_a;
           float best = pr[0];
           for (int cc = 1; cc < n_a; ++cc) { const float pvv = pr[cc]; if (pvv > best) { best = pvv; am = cc; } }

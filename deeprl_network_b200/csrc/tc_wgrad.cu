@@ -263,7 +263,7 @@ __global__ void __launch_bounds__(256) tc_wgrad_reduce_kernel(const __grid_const
       else if (ln > d.ka_cnt) { if (n >= NH && n < 2 * NH) grads[ag.o_w_fp + (ln - d.ka_cnt - 1) * NH + n - NH] = s; }   // fingerprint lanes
       else if (n < NH) grads[ag.o_b_ob + n] = s;                                       // ones lane: biases
       else if (m.variant == NMARL_NC && n < 2 * NH) grads[ag.o_b_fp + n - NH] = s;
-      else grads[ag.o_b_msg + n - ((m.variant == NMARL_NC) ? 2 * NH : NH)] = s;
+      else if (ag.o_b_msg >= 0) grads[ag.o_b_msg + n - ((m.variant == NMARL_NC) ? 2 * NH : NH)] = s;
     } else grads[ag.o_w_msg + (size_t)(128 * (kind - J_ENC_M0) + ln) * NH + n] = s;
   }
 }

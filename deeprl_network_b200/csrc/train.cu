@@ -326,7 +326,9 @@ __global__ void __launch_bounds__(256) wgrad_kernel(const __grid_constant__ WgK 
   float (*Ds)[RC][ND] = reinterpret_cast<float (*)[RC][ND]>(wg_smem + 2 * RC * 64);
   const int sp = blockIdx.x, mt = blockIdx.y, i = blockIdx.z;
   const int Ka = k.Ka[i];
-  if (mt * 64 >= Ka) return;
+  // mt == 0 always runs: it writes the bias row, which wgrad_reduce_kernel reads even when Ka == 0 (an agent without
+  // neighbours has no fingerprint / message inputs, but its encoder biases still get the column sums of D)
+  if (mt > 0 && mt * 64 >= Ka) return;
   const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
   const int R = k.T * k.B;
   const int per = ((R + k.splits - 1) / k.splits + RC - 1) / RC * RC;
@@ -777,11 +779,10 @@ int run_wgrad(const nmarl_model* m, const nmarl_bwd_args* a, int ngrp, const flo
   k.A = A; k.lda = lda; k.a_col0 = a_col0; k.D = D; k.ldd = ldd; k.d_col0 = d_col0;
   int kmax = 0;
   for (int i = 0; i < m->n_agent; ++i) { k.Ka[i] = Ka[i]; kmax = Ka[i] > kmax ? Ka[i] : kmax; }
-  if (kmax == 0) return 0;
   k.ka_max = kmax; k.ws = a->ws;
   const int nd = 64 * ngrp;
   NMARL_CHECK((int64_t)k.splits * k.N * (kmax + 1) * nd <= a->ws_floats, "wgrad: workspace too small");
-  dim3 grid(k.splits, (kmax + 63) / 64, m->n_agent);
+  dim3 grid(k.splits, kmax > 0 ? (kmax + 63) / 64 : 1, m->n_agent);     // kmax == 0: the bias rows only
   const size_t smem = (size_t)(2 * 32 * 64 + 2 * 32 * nd) * sizeof(float);
   static bool configured = false;
   if (!configured) {

@@ -306,7 +306,8 @@ class HeteroLayout(ModelLayout):
         d(logit) = pi * (g - <pi, g>) = 0, it is never sampled (its cdf step has zero width) and never the arg-max;
       * value-head rows of padded actions are never selected by a one-hot;
       * an agent without neighbours keeps zero message / fingerprint encoders (relu(0) = 0 feeds the gate GEMM
-        zeros and receives zero gradients -- the same argument as for ia2c_fp, see the module docstring).
+        zeros and receives zero gradients -- the same argument as for ia2c_fp, see the module docstring); a DIAL
+        one also drops the one-hot of its own last action (o_b_msg = -1), as lstm_dial_hetero does.
     Zero gradients leave clip-by-global-norm and RMSProp untouched, so pi, v, gradients and trained weights equal
     the reference's tight model.  pack / unpack / creation_order / checkpoints speak the reference's tight tensors.
     """
@@ -320,6 +321,12 @@ class HeteroLayout(ModelLayout):
         if variant == 'ma2c_ic3' and min(len(x) for x in self.nbr) == 0:
             raise NotImplementedError('CommNet agent without neighbours (mean over an empty set) is not supported')
         self.hetero = True
+        if variant == 'ma2c_dial':
+            # lstm_dial_hetero gives an agent without neighbours s = relu(x w_ob + b_ob) alone: no message term and no
+            # one-hot of its own last action (agents/utils.py:683-685).  The kernels drop both when o_b_msg = -1.
+            for i in range(self.N):
+                if not self.nbr[i]:
+                    self.agents_off[i]['o_b_msg'] = -1
         self._embed()
 
     def _embed(self):

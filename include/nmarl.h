@@ -50,7 +50,10 @@ typedef struct {
   /* offsets (floats, multiples of 4) into the flat parameter / gradient / rmsprop buffers; -1 = absent */
   int32_t o_w_ob, o_b_ob;                /* obs encoder  (IA2C: lstm_i/fc)                      */
   int32_t o_w_fp, o_b_fp;                /* fingerprint encoder (NC)                            */
-  int32_t o_w_msg, o_b_msg;              /* message encoder (NC, IC3, DIAL)                     */
+  int32_t o_w_msg, o_b_msg;              /* message encoder (NC, IC3, DIAL).  DIAL, agent without  */
+                                         /*   neighbours: o_b_msg = -1 drops the message AND the  */
+                                         /*   own-action one-hot from s (lstm_dial_hetero,        */
+                                         /*   agents/utils.py:683-685); lstm_dial keeps both      */
   int32_t o_wxh;                         /* [s_dim + 64][256] = wx rows then wh rows            */
   int32_t o_b;                           /* [256]                                               */
   int32_t o_mfc_w, o_mfc_b;              /* DIAL sender-side message fc                         */

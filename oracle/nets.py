@@ -197,6 +197,10 @@ class OraclePolicy:
         """x: list of N [B,n_s_i]; p: [B,N,n_a] or None; done [B]; c,h [B,N,n_h]."""
         nd = (1.0 - done).unsqueeze(-1)
         v = self.variant
+
+        def cat(parts):
+            # an agent without neighbours concatenates nothing: a [B, 0] input meets the reference's [0, n_h] weights
+            return torch.cat(parts, dim=1) if parts else torch.zeros(c.shape[0], 0, dtype=self.dtype)
         if v == 'ma2c_dial':   # sender-side message fc on the UN-masked h (agents/utils.py:563-566)
             sc = SCOPE[v]
             msg = [torch.relu(h[:, j] @ self.p['%s/mfc_%d/w' % (sc, j)] + self.p['%s/mfc_%d/b' % (sc, j)])
@@ -212,7 +216,7 @@ class OraclePolicy:
                 n_x = self.n_s_ls[i] - self.n_a * len(nb)
                 # the environment attaches the fingerprints to the observation; tests that keep them in a
                 # separate array pass observations of width n_x plus ps
-                fp_in = x[i][:, n_x:] if x[i].shape[1] > n_x else torch.cat([p[:, j] for j in nb], dim=1)
+                fp_in = x[i][:, n_x:] if x[i].shape[1] > n_x else cat([p[:, j] for j in nb])
                 hx = torch.relu(x[i][:, :n_x] @ self._w(i, 'fcs/w') + self._w(i, 'fcs/b'))
                 hp = torch.relu(fp_in @ self._w(i, 'fcp/w') + self._w(i, 'fcp/b'))
                 s = torch.cat([hx, hp], dim=1)
@@ -226,8 +230,8 @@ class OraclePolicy:
                 xi = torch.cat([x[i][:, :self.n_s_ls[i]]] + [x[j][:, :self.n_s_ls[j]] for j in nb], dim=1)
                 wx, wh, b = self._w(i, 'wx_hid'), self._w(i, 'wh_hid'), self._w(i, 'b_hid')
                 if v == 'ma2c_nc':
-                    mi = torch.cat([h[:, j] for j in nb], dim=1)
-                    pi_in = torch.cat([p[:, j, :self.n_a_ls[j]] for j in nb], dim=1)
+                    mi = cat([h[:, j] for j in nb])
+                    pi_in = cat([p[:, j, :self.n_a_ls[j]] for j in nb])
                     hx = torch.relu(xi @ self._w(i, 'w_ob') + self._w(i, 'b_ob'))
                     hp = torch.relu(pi_in @ self._w(i, 'w_fp') + self._w(i, 'b_fp'))
                     hm = torch.relu(mi @ self._w(i, 'w_msg') + self._w(i, 'b_msg'))
@@ -236,7 +240,7 @@ class OraclePolicy:
                     mi = torch.stack([h[:, j] for j in nb], dim=0).mean(dim=0)
                     s = torch.tanh(xi @ self._w(i, 'w_ob') + self._w(i, 'b_ob')) + mi @ self._w(i, 'w_msg') + self._w(i, 'b_msg')
                 else:  # dial
-                    mi = torch.cat([msg[j] for j in nb], dim=1)
+                    mi = cat([msg[j] for j in nb])
                     ai = torch.nn.functional.one_hot(torch.argmax(p[:, i], dim=1), self.n_h).to(self.dtype)
                     hx = torch.relu(xi @ self._w(i, 'w_ob') + self._w(i, 'b_ob'))
                     hm = torch.relu(mi @ self._w(i, 'w_msg') + self._w(i, 'b_msg'))

@@ -336,9 +336,16 @@ def tfnet_case(ini, total_step):
 # ---- heterogeneous agents (SURVEY 8 f4): lstm_comm_hetero / lstm_ic3_hetero / lstm_dial_hetero ---------------------
 HETERO = dict(edges=[(0, 1), (1, 2), (2, 3), (3, 4), (4, 5), (1, 4)],
               n_s_ls=[5, 7, 4, 6, 5, 3], n_a_ls=[4, 3, 5, 2, 4, 3], n_step=8, updates=3)
+# the same agents with one of them cut off (no neighbour; lstm_comm_hetero / lstm_dial_hetero then create no message /
+# fingerprint encoder for it, agents/utils.py:255-277).  CommNet is left out: its mean over no neighbours is undefined.
+HETERO_ISO = {'hetero_iso_': [(0, 1), (1, 2), (2, 3), (3, 4), (1, 4)],        # agent 5, the last one
+              'hetero_iso0_': [(1, 2), (2, 3), (3, 4), (4, 5), (1, 4)]}       # agent 0, the first one
+# These fixtures keep the trained weights of W1_SAMPLE entries per tensor (every entry of a smaller tensor), so that
+# they stay small: 'w1idx/<name>' = flat indices, 'w1/<name>' = the values there.  The pi / v / R trace stays complete.
+W1_SAMPLE = 256
 
 
-def hetero_case(agent):
+def hetero_case(agent, edges=HETERO['edges'], w1_sample=None):
     """The UNMODIFIED reference agent / policy / layer code for agents with UNEQUAL observation and action widths
     (agents/utils.py:220-341, 420-512, 602-702; agents/models.py:89-97, 229-235; agents/policies.py:289, 453, 502)
     on the TF shim.  CACC agents are identical, so a scripted stream stands in for the environment: random
@@ -354,7 +361,7 @@ def hetero_case(agent):
     H = HETERO
     N = len(H['n_s_ls'])
     mask = np.zeros((N, N), dtype=int)
-    for a, b in H['edges']:
+    for a, b in edges:
         mask[a, b] = mask[b, a] = 1
     dist = np.zeros((N, N), dtype=int)
     cp = _cfg('config_ma2c_nc_catchup.ini')
@@ -410,7 +417,12 @@ def hetero_case(agent):
     for n in w0:
         out['w0sha/' + n] = hashlib.sha256(np.ascontiguousarray(w0[n]).tobytes()).hexdigest()
         out['w0shape/' + n] = np.array(w0[n].shape)
-        out['w1/' + n] = w1[n]
+        if w1_sample is None or w1[n].size <= w1_sample:
+            out['w1/' + n] = w1[n]
+        else:
+            idx = np.sort(np.random.RandomState(len(out)).choice(w1[n].size, w1_sample, replace=False)).astype(np.int32)
+            out['w1idx/' + n] = idx
+            out['w1/' + n] = np.ascontiguousarray(w1[n]).ravel()[idx]
     return out
 
 
@@ -488,6 +500,14 @@ def main():
         out = hetero_case(agent)
         np.savez_compressed(os.path.join(HERE, name + '.npz'), **out)
         print(name, 'trace', out['trace'].shape, 'n_var', len(out['names']))
+    for prefix, edges in HETERO_ISO.items():
+        for agent in ('ma2c_nc', 'ma2c_dial'):
+            name = prefix + agent
+            if os.path.exists(os.path.join(HERE, name + '.npz')) and '--force' not in sys.argv:
+                continue
+            out = hetero_case(agent, edges, w1_sample=W1_SAMPLE)
+            np.savez_compressed(os.path.join(HERE, name + '.npz'), **out)
+            print(name, 'trace', out['trace'].shape, 'n_var', len(out['names']))
     if '--force' not in sys.argv:
         return
     for name, alpha, multi in [('buffer_ma_global', -1, True), ('buffer_ma_spatial09', 0.9, True),

@@ -27,6 +27,21 @@ def make_pair(variant, B, T=4, seed=0, dtype=torch.float32, mask=None, n_a=4, hp
     return eng, orc, lay, params
 
 
+def check_apply_twice(eng, orc, lay, pad, lr=1e-2):
+    """Two clip + RMSProp steps on the gradients of the last backward (the second one with ms != 1): norm_out equals
+    the oracle's global norm(s), the weights follow the oracle's, and every padding float (`pad`) stays exactly 0."""
+    for _ in range(2):
+        eng.apply(lr)
+        norms = orc.apply_grads(lr, max_grad_norm=HP['max_grad_norm'], alpha=HP['alpha'], epsilon=HP['epsilon'])
+        torch.cuda.synchronize()
+        np.testing.assert_allclose(eng.norm_out.cpu().numpy(), norms, rtol=1e-4)
+        flat = eng.params.cpu().numpy()
+        assert np.all(flat[pad] == 0), 'padding moved'
+        w = lay.unpack(flat)
+        for n in orc.names:
+            np.testing.assert_allclose(w[n], orc.p[n].detach().numpy(), rtol=0, atol=3e-6, err_msg=n)
+
+
 def oracle_obs(lay, base):
     """base [B, N, 5] own features -> per-agent oracle inputs (IA2C: own + neighbours concatenated)."""
     if lay.variant not in ('ia2c', 'ia2c_fp'):      # ia2c_fp: the fingerprints travel separately (ps)

@@ -3,26 +3,40 @@
     tests/golden/hetero_*.npz -- recorded from the UNMODIFIED reference MA2C_NC / MA2C_IC3 / MA2C_DIAL classes with
     n_s = [5,7,4,6,5,3], n_a = [4,3,5,2,4,3] on the TF shim -- and must reproduce every pi / v / R within 1e-5 and the
     weights after three updates within 2e-5, starting from the same NumPy-stream initial weights (exact).
+    The hetero_iso_* / hetero_iso0_* fixtures cut the last / the first agent off: it has no message or fingerprint
+    encoder, so its b_fp / b_msg (and for NeurComm wx_hid rows 64..191) are padding of the embedding and must stay
+    exactly 0; a DIAL agent without neighbours also adds no one-hot of its own action (lstm_dial_hetero).
 (2) The batched kernels (FFMA and tensor-core paths) against the batched oracle: pi / v / state 1e-5, gradients
-    2e-5 x scale against float64 autograd, and the zero-padding of the embedding receives exactly zero gradient."""
+    2e-5 x scale against float64 autograd, and the zero-padding of the embedding receives exactly zero gradient;
+    then two optimizer steps: norm_out equals the oracle's global norm and the padding stays exactly 0."""
 import hashlib
 
 import numpy as np
 import pytest
 import torch
 
-from gpu_common import HP, bn, nb, to_dev
+from gpu_common import HP, bn, check_apply_twice, nb, to_dev
 from helpers import golden, load_cfg, random_params
 from oracle import nets
-from test_hetero_parity import AGENTS, replay
+from test_hetero_parity import GOLDEN, replay, variant_of, w1_error
 
 pytestmark = pytest.mark.gpu
 
 
-@pytest.mark.parametrize('agent', AGENTS)
-def test_drop_in_agent_follows_reference_hetero_golden(agent):
+def _padding(lay):
+    """flat-buffer floats that belong to no reference tensor and are not a padded action's bias: exactly 0 for good"""
+    pad = np.ones(lay.n_param, bool)
+    for n in lay._idx:
+        pad[lay._idx[n]] = False
+    pad[lay.pi_pad] = False
+    return pad
+
+
+@pytest.mark.parametrize('name', GOLDEN)
+def test_drop_in_agent_follows_reference_hetero_golden(name):
     from deeprl_network_b200.agents.models import MA2C_DIAL, MA2C_IC3, MA2C_NC
-    g = golden('hetero_' + agent)
+    agent = variant_of(name)
+    g = golden(name)
     mc = load_cfg('config_ma2c_nc_catchup.ini')['MODEL_CONFIG']
     mc['batch_size'] = str(int(g['n_step']))
     n_s, n_a = [int(x) for x in g['n_s_ls']], [int(x) for x in g['n_a_ls']]
@@ -42,15 +56,18 @@ def test_drop_in_agent_follows_reference_hetero_golden(agent):
     assert np.abs(trace - g['trace']).max() < 1e-5
     w1 = m.get_weights()
     for n in names:
-        assert np.abs(w1[n] - g['w1/' + n]).max() < 2e-5, n
+        assert w1_error(g, n, w1[n]) < 2e-5, n
     flat = m.engine.params.cpu().numpy()
     assert np.all(flat[m.layout.pi_pad] == np.float32(-1e30))           # padded actions never moved
+    # the rest of the padding -- an isolated agent's b_fp / b_msg and unused wx_hid rows included -- never moved either
+    assert np.all(flat[_padding(m.layout)] == 0)
 
 
-def _pair(agent, B, T):
+def _pair(name, B, T):
     from deeprl_network_b200.agents.engine import PolicyEngine
     from deeprl_network_b200.layout import HeteroLayout
-    g = golden('hetero_' + agent)
+    agent = variant_of(name)
+    g = golden(name)
     n_s, n_a, mask = [int(x) for x in g['n_s_ls']], [int(x) for x in g['n_a_ls']], g['mask']
     lay = HeteroLayout(agent, n_s, n_a, mask)
     params = random_params(lay.creation_order(), seed=2, scale=0.3)
@@ -70,11 +87,11 @@ def _inputs(rs, shape, n_s, n_a):
     return ob, fp
 
 
-@pytest.mark.parametrize('agent', AGENTS)
+@pytest.mark.parametrize('name', GOLDEN)
 @pytest.mark.parametrize('B', [7, 128])                     # 128: tensor-core path
-def test_hetero_kernels_match_oracle(agent, B):
+def test_hetero_kernels_match_oracle(name, B):
     T = 4
-    eng, orc, lay, n_s, n_a = _pair(agent, B, T)
+    eng, orc, lay, n_s, n_a = _pair(name, B, T)
     assert eng.use_tc == (B % 128 == 0)
     N = len(n_s)
     rs = np.random.RandomState(1)
@@ -125,3 +142,4 @@ def test_hetero_kernels_match_oracle(agent, B):
     for n in orc.names:
         used[lay._idx[n]] = True
     assert np.all(flat[~used] == 0)                           # the zero-padding of the embedding gets zero gradient
+    check_apply_twice(eng, orc, lay, _padding(lay))

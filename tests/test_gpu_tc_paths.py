@@ -63,6 +63,9 @@ VARIANTS = ['ma2c_nc', 'ma2c_ic3', 'ma2c_dial', 'ia2c', 'ia2c_fp', 'ma2c_cu']
 CASES = []
 
 
+CUT = 3                         # topo 'chain8cut': the agent without neighbours
+
+
 def _case(cid, variant, B, T, purpose, topo='chain8', n_a=4, dones='mixed', kb=None):
     CASES.append(pytest.param(dict(variant=variant, B=B, T=T, topo=topo, n_a=n_a, dones=dones, kb=kb, purpose=purpose),
                               id=cid))
@@ -71,8 +74,13 @@ def _case(cid, variant, B, T, purpose, topo='chain8', n_a=4, dones='mixed', kb=N
 for _v in VARIANTS:
     _case('variant-' + _v, _v, 256, 8, 'every variant on the 8-agent chain, two 128-env tiles')
 for _v in ('ma2c_nc', 'ma2c_ic3', 'ma2c_dial'):
-    _case('hetero-' + _v, _v, 256, 8, 'unequal n_s / n_a and agents without neighbours (tests/golden/hetero_*)',
-          topo='hetero')
+    _case('hetero-' + _v, _v, 256, 8, 'unequal n_s / n_a on an irregular graph (tests/golden/hetero_*)', topo='hetero')
+for _v in ('ma2c_nc', 'ma2c_dial'):
+    _case('hetero-iso-' + _v, _v, 256, 8, 'unequal n_s / n_a, the last agent without neighbours: no fingerprint / '
+          'message k-blocks (tests/golden/hetero_iso_*)', topo='hetero_iso')
+for _v in ('ma2c_nc', 'ia2c_fp'):
+    _case('isolated-' + _v, _v, 256, 8, '8-agent chain with agent %d cut off: [0, 64] fingerprint / message weights '
+          'and non-zero b_fp / b_msg' % CUT, topo='chain8cut')
 for _v in ('ma2c_nc', 'ma2c_ic3'):
     _case('done-t0-' + _v, _v, 256, 8, 'every env done at t = 0: the non-zero initial state is masked out', dones='t0')
     _case('done-block-' + _v, _v, 256, 8, 'one whole 32-row block (one gate-bias partial) done mid-sequence',
@@ -121,7 +129,7 @@ class RoundoffScale(TorchFunctionMode):
             d[n] += val
 
     def _rows(self, t):
-        return t.reshape(-1, t.shape[-1])
+        return t.reshape(int(np.prod(t.shape[:-1])), t.shape[-1])     # also [B, 0]: an empty neighbour input
 
     def __torch_function__(self, func, types, args=(), kwargs=None):
         out = func(*args, **(kwargs or {}))
@@ -165,12 +173,14 @@ def _model(c):
     from deeprl_network_b200.envs.cacc_env import grid_masks
     from deeprl_network_b200.layout import HeteroLayout, ModelLayout
     v = c['variant']
-    if c['topo'] == 'hetero':
-        g = golden('hetero_' + v)
+    if c['topo'].startswith('hetero'):
+        g = golden(c['topo'] + '_' + v)
         n_s, n_a, mask = [int(x) for x in g['n_s_ls']], [int(x) for x in g['n_a_ls']], g['mask']
         lay = HeteroLayout(v, n_s, n_a, mask)
         return lay, (v, n_s, n_a, mask), n_s, n_a
     mask = grid_masks(5)[0] if c['topo'] == 'grid5' else chain_masks(32 if c['topo'] == 'chain32' else 8)[0]
+    if c['topo'] == 'chain8cut':
+        mask[CUT, :] = 0; mask[:, CUT] = 0
     N, n_a = len(mask), c['n_a']
     nm = [int(mask[i].sum()) for i in range(N)]
     n_s_ls = {'ia2c': [5 * (1 + k) for k in nm], 'ia2c_fp': [5 * (1 + k) + n_a * k for k in nm]}.get(v, [5] * N)
@@ -292,7 +302,7 @@ def _run_fused(e, lay, x, W):
 def _oracle(lay, orc_args, params, c, x, n_s, fp, acts):
     T, B, N = c['T'], c['B'], len(n_s)
     orc = nets.OraclePolicy(*orc_args, params=params, dtype=torch.float64, n_env=B)
-    if c['topo'] == 'hetero':
+    if c['topo'].startswith('hetero'):
         obs = [[x['base'][t][:, i, :n_s[i]] for i in range(N)] for t in range(T)]
     else:
         obs = [oracle_obs(lay, x['base'][t]) for t in range(T)]
@@ -340,6 +350,8 @@ def _check(tag, r, ref, used):
     """per-tensor checks of one run against the oracle; returns {tensor: per-entry ratio max|g - g64| / S}"""
     ratios = {}
     for n, g64 in ref['g'].items():
+        if g64.size == 0:              # the [0, 64] fingerprint / message weights of an agent without neighbours
+            continue
         err = np.maximum(np.abs(r['g'][n] - g64) - ref['K'][n], 0)        # minus what a ReLU kink may flip
         scale = max(1e-3, np.abs(g64).max())
         assert err.max() <= 2e-5 * scale + 1e-7, (tag, n, err.max(), scale)
@@ -367,6 +379,8 @@ def test_tc_paths_match_fp64(c, monkeypatch):
         assert [min(SEG_KB, per - s) for s in range(0, per, SEG_KB)] == c['kb'][1]
     if c['topo'] == 'chain32':
         assert wgrad_splits(N) == 5
+    if c['topo'] in ('hetero_iso', 'chain8cut'):
+        assert [i for i in range(N) if lay.nbr[i] == []] == [N - 1 if c['topo'] == 'hetero_iso' else CUT]
     if c['topo'] == 'grid5':
         assert wgrad_splits(N) == 9 and sorted({int(k) for k in orc_args[3].sum(1)}) == [2, 3, 4]
     params = random_params(lay.creation_order(), seed=3, scale=0.3)
