@@ -67,9 +67,9 @@ __device__ __forceinline__ JobDesc job_desc(const nmarl_model& m, const TcWgK& k
   return d;
 }
 
-// RAW: the D^T tiles hold raw fp32 once.  One tile per k-block is copied into the hi half of the stage; the MMA
-// warpgroup splits it in place into the same rounded [hi | lo] pair the packed tiles carry (tc::split_tf32) before
-// the k-block's MMAs.
+// RAW: the D^T tiles hold raw fp32 once.  One tile per k-block is copied into the hi half of the stage; the A-producer
+// threads split it in place into the same rounded [hi | lo] pair the packed tiles carry (tc::split_tf32) and signal
+// b_split, so the split overlaps the previous k-block's MMAs instead of preceding the k-block's own.
 template <bool RAW>
 __global__ void __launch_bounds__(WG_THREADS, 1) tc_wgrad_kernel(const __grid_constant__ nmarl_model m,
                                                                  const __grid_constant__ TcWgK k) {
@@ -78,7 +78,8 @@ __global__ void __launch_bounds__(WG_THREADS, 1) tc_wgrad_kernel(const __grid_co
   uint8_t* bst = smem;
   uint8_t* ast = smem + (size_t)WG_STAGES * STAGE_BYTES;
   uint64_t* bars = reinterpret_cast<uint64_t*>(ast + A_SLOTS * A_SLOT_BYTES);
-  uint64_t* b_full = bars, *a_full = bars + WG_STAGES, *a_empty = a_full + A_SLOTS;
+  uint64_t* b_full = bars, *a_full = bars + WG_STAGES, *a_empty = a_full + A_SLOTS, *b_split = a_empty + A_SLOTS;
+  static_assert(2 * WG_STAGES + 2 * A_SLOTS <= 16, "mbarrier area of WG_SMEM");
 
   const int sp = blockIdx.x, jslot = blockIdx.y >> 1, mh = blockIdx.y & 1, i = blockIdx.z;
   const int kind = k.jobs[jslot];
@@ -95,6 +96,7 @@ __global__ void __launch_bounds__(WG_THREADS, 1) tc_wgrad_kernel(const __grid_co
   if (tid == 0) {
     for (int s = 0; s < WG_STAGES; ++s) tc::mbar_init(&b_full[s], 1);
     for (int s = 0; s < A_SLOTS; ++s) { tc::mbar_init(&a_full[s], WG_A_THREADS); tc::mbar_init(&a_empty[s], 128); }
+    for (int s = 0; s < WG_STAGES; ++s) tc::mbar_init(&b_split[s], WG_A_THREADS);
     tc::fence_barrier_init();
   }
   __syncthreads();
@@ -167,6 +169,24 @@ __global__ void __launch_bounds__(WG_THREADS, 1) tc_wgrad_kernel(const __grid_co
       tc::fence_proxy_async();
       tc::mbar_arrive(&a_full[slot]);
       if (q + 2 < nkb) load_x(q + 2, x);        // refill this buffer; it is consumed two k-blocks from now
+      if constexpr (RAW) {
+        // split the raw D^T tile of this k-block into its [hi | lo] pair once it has landed.  In order: the stage is
+        // refilled with k-block q + WG_STAGES only after the MMAs of q, which wait for this split, have retired.
+        const int st = q % WG_STAGES;
+        tc::mbar_wait(&b_full[st], (q / WG_STAGES) & 1, k.err, 31);
+        float4* bhi = reinterpret_cast<float4*>(bst + (size_t)st * STAGE_BYTES);
+        float4* blo = reinterpret_cast<float4*>(bst + (size_t)st * STAGE_BYTES + tile_bytes);
+        for (uint32_t e = (uint32_t)tid; e < tile_bytes / 16; e += WG_A_THREADS) {
+          const float4 v = bhi[e];
+          float4 h, lo4;
+          tc::split_tf32(v.x, h.x, lo4.x); tc::split_tf32(v.y, h.y, lo4.y);
+          tc::split_tf32(v.z, h.z, lo4.z); tc::split_tf32(v.w, h.w, lo4.w);
+          bhi[e] = h;
+          blo[e] = lo4;
+        }
+        tc::fence_proxy_async();
+        tc::mbar_arrive(&b_split[st]);
+      }
     };
     if (nkb > 0) load_x(0, xa);
     if (nkb > 1) load_x(1, xb);
@@ -213,21 +233,8 @@ __global__ void __launch_bounds__(WG_THREADS, 1) tc_wgrad_kernel(const __grid_co
       const int st = q % WG_STAGES, slot = q & (A_SLOTS - 1);
       const bool seg_first = (q % SEG_KB) == 0;
       uint8_t* b = bst + (size_t)st * STAGE_BYTES;
-      tc::mbar_wait(&b_full[st], (q / WG_STAGES) & 1, k.err, 31);
-      if constexpr (RAW) {
-        float4* hi = reinterpret_cast<float4*>(b);
-        float4* lo = reinterpret_cast<float4*>(b + tile_bytes);
-        for (uint32_t e = (uint32_t)t; e < tile_bytes / 16; e += 128) {
-          const float4 v = hi[e];
-          float4 h, lo4;
-          tc::split_tf32(v.x, h.x, lo4.x); tc::split_tf32(v.y, h.y, lo4.y);
-          tc::split_tf32(v.z, h.z, lo4.z); tc::split_tf32(v.w, h.w, lo4.w);
-          hi[e] = h;
-          lo[e] = lo4;
-        }
-        tc::fence_proxy_async();
-        mma_wg_sync();
-      }
+      if constexpr (RAW) tc::mbar_wait(&b_split[st], (q / WG_STAGES) & 1, k.err, 33);   // landed and split (A producers)
+      else tc::mbar_wait(&b_full[st], (q / WG_STAGES) & 1, k.err, 31);
       tc::mbar_wait(&a_full[slot], (q / A_SLOTS) & 1, k.err, 32);
       uint8_t* a = ast + slot * A_SLOT_BYTES;
       tc::wgmma_fence();
