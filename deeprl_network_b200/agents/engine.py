@@ -319,10 +319,11 @@ class PolicyEngine:
                                                0 if self.alpha_pow is None else self.alpha_pow.numel(),
                                                L.ptr(self.Rs), L.ptr(self.Advs), L.stream()), 'nmarl_nstep_return_adv')
         self.launches += 1
-        if getattr(self.layout, 'hetero', False):
+        if getattr(self.layout, 'hetero', False) and not self.model.per_agent_norm:
             # Reference quirk Q7 (agents/policies.py:241-251, non-identical branch): prob_pi [N,1,T] * ADV [N,T]
             # broadcasts to [N,N,T], so agent i's log-probability is weighted by the SUM over agents of the
-            # advantages.  Reproduced for parity with the reference's heterogeneous-agent path.
+            # advantages.  Reproduced for parity with the reference's heterogeneous-agent path.  IA2C / IA2C_FP
+            # have one loss per agent (Policy.prepare_loss, agents/policies.py:20-30) and no such broadcast.
             self.Advs[:T] = self.Advs[:T].sum(dim=1, keepdim=True).expand(-1, self.N, -1)
 
     # ---- training -------------------------------------------------------------------------------------

@@ -42,9 +42,6 @@ class IA2C:
         if self.identical_agent:
             self.n_s, self.n_a = self.n_s_ls[0], self.n_a_ls[0]
         else:
-            if self.variant not in ('ma2c_nc', 'ma2c_ic3', 'ma2c_dial'):
-                raise NotImplementedError('heterogeneous action spaces are covered for ma2c_nc / ma2c_ic3 / ma2c_dial '
-                                          '(lstm_comm_hetero / lstm_ic3_hetero / lstm_dial_hetero)')
             self.n_s, self.n_a = max(self.n_s_ls), max(self.n_a_ls)
         self.neighbor_mask = np.asarray(neighbor_mask)
         self.n_agent = len(self.neighbor_mask)
@@ -55,15 +52,22 @@ class IA2C:
         self.n_lstm = model_config.getint('num_lstm')
         self.n_env = int(n_env)
         self.sess = None
+        if not self.identical_agent and self.variant in ('ia2c', 'ia2c_fp') and obs_mode not in (None, 'concat'):
+            raise ValueError('heterogeneous %s agents read their own observation rows as given (obs_mode concat)'
+                             % self.variant)
         if obs_mode is None:
             obs_mode = 'concat' if self.variant == 'ia2c' else 'gather'
-        if self.variant == 'ia2c_fp':     # "neighborhood policies are included in local state" (agents/models.py:172-177)
-            self.n_s_ls = [n + self.n_a * int(np.sum(self.neighbor_mask[i])) for i, n in enumerate(self.n_s_ls)]
+        own_n_s_ls = list(self.n_s_ls)
+        if self.variant == 'ia2c_fp':     # "neighborhood policies are included in local state" (agents/models.py:172-188)
+            self.n_s_ls = [n + sum(self.n_a_ls[j] for j in np.where(self.neighbor_mask[i] == 1)[0])
+                           for i, n in enumerate(self.n_s_ls)]
         if self.identical_agent:
             self.layout = ModelLayout(self.variant, self.n_s_ls, self.n_a, self.neighbor_mask,
                                       n_h=self.n_lstm, n_fc=self.n_fc, obs_mode=obs_mode)
         else:
-            self.layout = HeteroLayout(self.variant, self.n_s_ls, self.n_a_ls, self.neighbor_mask,
+            # IA2C / IA2C_FP read each agent's own observation row as given (IA2C_FP: the part in front of the
+            # fingerprints); the MA2C family and IA2C_CU pad it to max(n_s_ls)
+            self.layout = HeteroLayout(self.variant, own_n_s_ls, self.n_a_ls, self.neighbor_mask,
                                        n_h=self.n_lstm, n_fc=self.n_fc)
         self.nbr = self.layout.nbr
         hp = dict(v_coef=0.5, e_coef=0.01, max_grad_norm=40.0, alpha=0.99, epsilon=1e-5, gamma=0.99,
@@ -98,7 +102,12 @@ class IA2C:
         out = np.zeros((self.n_agent, S), dtype=np.float32)
         for i in range(self.n_agent):
             o = np.asarray(obs[i], dtype=np.float32).ravel()
-            w = min(len(o), self.layout.base_n_s) if self.layout.obs_mode == 'gather' else len(o)
+            if self.layout.obs_mode == 'gather':
+                w = min(len(o), self.layout.base_n_s)
+            elif self.variant == 'ia2c_fp':     # heterogeneous IA2C_FP: the fingerprints behind it go to _ps_from_obs
+                w = self.layout.n_s_ls[i]
+            else:
+                w = len(o)
             out[i, :w] = o[:w]              # shorter rows (heterogeneous agents) stay zero-padded (agents/models.py:229-235)
         return out
 
@@ -120,7 +129,7 @@ class IA2C:
         if out_type.startswith('p'):
             e.step_p(s['obs'], fp, s['done'], e.pi_tmp)
             pi = e.pi_tmp[:, 0].cpu().numpy()
-            return [pi[i] for i in range(self.n_agent)]
+            return [pi[i, :self.n_a_ls[i]] for i in range(self.n_agent)]      # heterogeneous agents: tight widths
         a = np.zeros(self.n_agent, dtype=np.int32)
         for i in range(self.n_agent):
             for k, j in enumerate(self.nbr[i]):
@@ -245,10 +254,23 @@ class IA2C_FP(IA2C):
     """Fingerprint IA2C (agents/models.py:161-188): FPPolicy encodes the neighbours' last policies, which the
     environment appends to each observation (envs/cacc_env.py:74-77), with a second fc layer.  The kernels
     gather observations and fingerprints per neighbour on the device, so the host splits the reference's
-    concatenated observation back into own features and one policy row per agent."""
+    concatenated observation back into own features and one policy row per agent.  With heterogeneous agents each
+    neighbour's fingerprint is n_a_ls[j] wide, and the own features are the first n_s_ls[i] entries as given."""
     variant = 'ia2c_fp'
 
     def _ps_from_obs(self, obs):
+        if not self.identical_agent:
+            # agent i's observation = its own n_s_ls[i] features, then neighbour j's policy (n_a_ls[j] wide) for every
+            # neighbour in ascending order (agents/models.py:181-184).  Rows are zero-padded to max(n_a_ls): a padded
+            # fingerprint entry must be exactly 0, as it meets fcp rows that are padding.
+            ps = np.zeros((self.n_agent, self.n_a), dtype=np.float32)
+            for i in range(self.n_agent):
+                o = np.asarray(obs[i], dtype=np.float32).ravel()
+                off = self.layout.n_s_ls[i]
+                for j in self.nbr[i]:
+                    ps[j, :self.n_a_ls[j]] = o[off: off + self.n_a_ls[j]]
+                    off += self.n_a_ls[j]
+            return ps
         ps = np.full((self.n_agent, self.n_a), 1.0 / self.n_a, dtype=np.float32)
         b = self.layout.base_n_s
         for i in range(self.n_agent):

@@ -68,7 +68,13 @@ class ModelLayout:
             raise ValueError('more than %d neighbours' % L.MAX_NBR)
         self.n_s_ls = [int(x) for x in n_s_ls]
         self.obs_mode = obs_mode
-        if variant == 'ia2c_fp':
+        self.concat = obs_mode == 'concat' and variant in ('ia2c', 'ia2c_fp')     # one source per agent, own width
+        if variant == 'ia2c_fp' and obs_mode == 'concat':
+            # heterogeneous agents (HeteroLayout): n_s_ls is the width of each agent's own pre-concatenated
+            # observation, which feeds fcs; the fingerprints are still gathered per neighbour on the device
+            assert getattr(self, 'hetero', False), 'ia2c_fp observations are gathered on the device'
+            self.base_n_s = None
+        elif variant == 'ia2c_fp':
             # n_s_ls counts own + neighbour observations + neighbour fingerprints (agents/models.py:175)
             assert obs_mode == 'gather', 'ia2c_fp observations are gathered on the device'
             self.base_n_s = int(base_n_s) if base_n_s else (self.n_s_ls[0] - n_a * len(self.nbr[0])) // (1 + len(self.nbr[0]))
@@ -89,7 +95,7 @@ class ModelLayout:
 
     # ------------------------------------------------------------------------------------------
     def _kx(self, i):
-        if self.variant == 'ia2c' and self.obs_mode == 'concat':
+        if self.concat:
             return self.n_s_ls[i]
         if self.variant == 'ma2c_cu':
             return self.base_n_s
@@ -193,7 +199,7 @@ class ModelLayout:
         self.kp_pad = _up4(n_a * max_nbr) if self.vid == L.NC else 0
         self.km_pad = {'ia2c': 0, 'ma2c_cu': 0, 'ma2c_ic3': NH}.get(v, NH * max_nbr)
         self.ld_in = self.kx_pad + self.kp_pad + self.km_pad
-        if v == 'ia2c' and self.obs_mode == 'concat':
+        if self.concat:
             self.obs_stride = _up4(max(self.n_s_ls))
         else:
             self.obs_stride = _up4(self.base_n_s)
@@ -219,7 +225,7 @@ class ModelLayout:
             ag.n_recv = len(recv[i])
             for s, (k, slot) in enumerate(recv[i]):
                 ag.recv_agent[s], ag.recv_slot[s] = k, slot
-            if self.variant == 'ia2c' and self.obs_mode == 'concat':
+            if self.concat:
                 ag.x_nsrc, ag.x_w = 1, self.n_s_ls[i]
                 ag.x_src[0] = i
             else:
@@ -296,7 +302,8 @@ PI_PAD_BIAS = -1.0e30      # bias of a padded (non-existent) action: softmax giv
 class HeteroLayout(ModelLayout):
     """Agents with UNEQUAL observation / action widths (the reference's ``identical_agent == False`` path:
     lstm_comm_hetero / lstm_ic3_hetero / lstm_dial_hetero, agents/utils.py:220-341, 420-512, 602-702; per-agent
-    heads, agents/policies.py:289-312; zero-padded inputs, agents/models.py:229-235).
+    heads, agents/policies.py:59-77, 289-312, 386; zero-padded inputs, agents/models.py:229-235; per-agent
+    LstmPolicy / FPPolicy with per-neighbour action widths, agents/models.py:118-132, 171-188).
 
     The kernels stay homogeneous: the model is EMBEDDED in a padded one with ``n_s = max(n_s_ls)`` and
     ``n_a = max(n_a_ls)`` for everybody.  Every reference tensor (tight shape, reference name, reference creation
@@ -310,17 +317,31 @@ class HeteroLayout(ModelLayout):
         one also drops the one-hot of its own last action (o_b_msg = -1), as lstm_dial_hetero does.
     Zero gradients leave clip-by-global-norm and RMSProp untouched, so pi, v, gradients and trained weights equal
     the reference's tight model.  pack / unpack / creation_order / checkpoints speak the reference's tight tensors.
+
+    Per variant:
+      * ma2c_nc / ma2c_ic3 / ma2c_dial: observations padded to n_s_max, gathered from the agent and its neighbours.
+      * ia2c / ia2c_fp: every agent reads the caller's own pre-concatenated observation of width n_s_ls[i]
+        (x_nsrc = 1, x_w = n_s_ls[i]; for ia2c_fp that is the part in front of the fingerprints, which feeds fcs), so
+        fc / fcs need no padding.  ia2c_fp gathers the neighbours' fingerprints, each n_a_max wide: fcp row
+        k * n_a_max + a is action a of the k-th neighbour.  An ia2c_fp agent without neighbours has no fcp and a
+        [64, 256] lstm/wx (rows 64..127 of the padded one, and b_fp, are padding).
+      * ma2c_cu: ConsensusPolicy pads every observation to n_s_max and fc_%da acts on the padded width, so its
+        tight fc_%da/w is the whole [n_s_max, 64] tensor.  Its policy head is named cu/pi_%da (agents/policies.py:386).
     """
 
     def __init__(self, variant, n_s_ls, n_a_ls, neighbor_mask, n_h=64, n_fc=64):
-        if variant not in SCOPE:
-            raise ValueError('heterogeneous agents exist for ma2c_nc / ma2c_ic3 / ma2c_dial only (got %r)' % variant)
+        if variant not in VARIANT_ID:
+            raise ValueError('unsupported agent %r' % variant)
         self.tight_n_s, self.tight_n_a = [int(x) for x in n_s_ls], [int(x) for x in n_a_ls]
         ns_max, na_max = max(self.tight_n_s), max(self.tight_n_a)
-        super().__init__(variant, [ns_max] * len(self.tight_n_s), na_max, neighbor_mask, n_h=n_h, n_fc=n_fc, obs_mode='gather')
+        self.hetero = True
+        if variant in PER_AGENT_OPT:
+            super().__init__(variant, self.tight_n_s, na_max, neighbor_mask, n_h=n_h, n_fc=n_fc, obs_mode='concat')
+        else:
+            super().__init__(variant, [ns_max] * len(self.tight_n_s), na_max, neighbor_mask, n_h=n_h, n_fc=n_fc,
+                             obs_mode='gather')
         if variant == 'ma2c_ic3' and min(len(x) for x in self.nbr) == 0:
             raise NotImplementedError('CommNet agent without neighbours (mean over an empty set) is not supported')
-        self.hetero = True
         if variant == 'ma2c_dial':
             # lstm_dial_hetero gives an agent without neighbours s = relu(x w_ob + b_ob) alone: no message term and no
             # one-hot of its own last action (agents/utils.py:683-685).  The kernels drop both when o_b_msg = -1.
@@ -342,46 +363,77 @@ class HeteroLayout(ModelLayout):
             idx[new_name] = (o + r[:, None] * pc + np.arange(ncol)[None, :]).ravel()
             tight.append((new_name, (len(r), ncol)))
 
-        def vec(name, n=None):
+        def vec(name, n=None, new_name=None):
             o, shp = pad[name]
             n = shp[0] if n is None else n
-            idx[name] = o + np.arange(n, dtype=np.int64)
-            tight.append((name, (n,)))
+            new_name = new_name or name
+            idx[new_name] = o + np.arange(n, dtype=np.int64)
+            tight.append((new_name, (n,)))
 
-        sc, cell = SCOPE[v], CELL[v]
-        for i in range(N):
-            s = '%s/%s_%d' % (sc, cell, i)
-            nb = self.nbr[i]
-            x_rows = [f for f in range(self.tight_n_s[i])] + [(k + 1) * ns_max + f for k, j in enumerate(nb) for f in range(self.tight_n_s[j])]
-            p_rows = [k * na_max + a for k, j in enumerate(nb) for a in range(self.tight_n_a[j])]
-            km = NH if v == 'ma2c_ic3' else NH * len(nb)
-            if v == 'ma2c_nc':           # creation order of lstm_comm_hetero: w_ob first (agents/utils.py:260-283)
-                rows(s + '/w_ob', s + '/w_ob', x_rows, NH); vec(s + '/b_ob')
-                if nb:
-                    rows(s + '/w_fp', s + '/w_fp', p_rows, NH); vec(s + '/b_fp')
-                    rows(s + '/w_msg', s + '/w_msg', range(km), NH); vec(s + '/b_msg')
-                rows(s + '/wx_hid', s + '/wx_hid', range(3 * NH if nb else NH), 4 * NH)
-            else:
-                if nb:
-                    rows(s + '/w_msg', s + '/w_msg', range(km), NH); vec(s + '/b_msg')
-                rows(s + '/w_ob', s + '/w_ob', x_rows, NH); vec(s + '/b_ob')
-                rows(s + '/wx_hid', s + '/wx_hid', range(NH), 4 * NH)
-            rows(s + '/wh_hid', s + '/wh_hid', range(NH), 4 * NH); vec(s + '/b_hid')
-        if v == 'ma2c_dial':
-            for i in range(N):
-                rows('dial/mfc_%d/w' % i, 'dial/mfc_%d/w' % i, range(NH), NH); vec('dial/mfc_%d/b' % i)
         self.pi_pad = []
-        for i in range(N):
-            hp, hv = '%s/pi_%d' % (sc, i), '%s/v_%d' % (sc, i)
+
+        def heads(i, hp, hv, tight_hp=None):
+            """the agent's n_a_i policy columns (padded actions get PI_PAD_BIAS); value head: h, then one one-hot
+            block per neighbour j with its n_a_j real rows at stride n_a_max"""
+            tight_hp = tight_hp or hp
             na = self.tight_n_a[i]
             o, _ = pad[hp + '/w']
-            idx[hp + '/w'] = (o + np.arange(NH)[:, None] * na_max + np.arange(na)[None, :]).ravel()
-            tight.append((hp + '/w', (NH, na)))
-            vec(hp + '/b', na)
+            idx[tight_hp + '/w'] = (o + np.arange(NH)[:, None] * na_max + np.arange(na)[None, :]).ravel()
+            tight.append((tight_hp + '/w', (NH, na)))
+            vec(hp + '/b', na, tight_hp + '/b')
             ob, _ = pad[hp + '/b']
             self.pi_pad += [ob + a for a in range(na, na_max)]
             v_rows = list(range(NH)) + [NH + k * na_max + a for k, j in enumerate(self.nbr[i]) for a in range(self.tight_n_a[j])]
             rows(hv + '/w', hv + '/w', v_rows, 1); vec(hv + '/b')
+
+        if v in PER_AGENT_OPT or v == 'ma2c_cu':
+            # one policy after the other, each with its own heads (agents/policies.py:136-185, 378-396)
+            for i in range(N):
+                nb = self.nbr[i]
+                if v == 'ma2c_cu':
+                    s = 'cu/'
+                    rows(s + 'fc_%da/w' % i, s + 'fc_%da/w' % i, range(ns_max), NH); vec(s + 'fc_%da/b' % i)
+                    lstm = s + 'lstm_%da' % i
+                else:
+                    s = 'lstm_%d/' % i
+                    enc = 'fc' if v == 'ia2c' else 'fcs'
+                    rows(s + enc + '/w', s + enc + '/w', range(self.tight_n_s[i]), NH); vec(s + enc + '/b')
+                    if v == 'ia2c_fp' and nb:
+                        p_rows = [k * na_max + a for k, j in enumerate(nb) for a in range(self.tight_n_a[j])]
+                        rows(s + 'fcp/w', s + 'fcp/w', p_rows, NH); vec(s + 'fcp/b')
+                    lstm = s + 'lstm'
+                n_in = 2 * NH if (v == 'ia2c_fp' and nb) else NH
+                rows(lstm + '/wx', lstm + '/wx', range(n_in), 4 * NH)
+                rows(lstm + '/wh', lstm + '/wh', range(NH), 4 * NH); vec(lstm + '/b')
+                if v == 'ma2c_cu':
+                    heads(i, 'cu/pi_%d' % i, 'cu/v_%da' % i, tight_hp='cu/pi_%da' % i)
+                else:
+                    heads(i, s + 'pi', s + 'v')
+        else:
+            sc, cell = SCOPE[v], CELL[v]
+            for i in range(N):
+                s = '%s/%s_%d' % (sc, cell, i)
+                nb = self.nbr[i]
+                x_rows = [f for f in range(self.tight_n_s[i])] + [(k + 1) * ns_max + f for k, j in enumerate(nb) for f in range(self.tight_n_s[j])]
+                p_rows = [k * na_max + a for k, j in enumerate(nb) for a in range(self.tight_n_a[j])]
+                km = NH if v == 'ma2c_ic3' else NH * len(nb)
+                if v == 'ma2c_nc':           # creation order of lstm_comm_hetero: w_ob first (agents/utils.py:260-283)
+                    rows(s + '/w_ob', s + '/w_ob', x_rows, NH); vec(s + '/b_ob')
+                    if nb:
+                        rows(s + '/w_fp', s + '/w_fp', p_rows, NH); vec(s + '/b_fp')
+                        rows(s + '/w_msg', s + '/w_msg', range(km), NH); vec(s + '/b_msg')
+                    rows(s + '/wx_hid', s + '/wx_hid', range(3 * NH if nb else NH), 4 * NH)
+                else:
+                    if nb:
+                        rows(s + '/w_msg', s + '/w_msg', range(km), NH); vec(s + '/b_msg')
+                    rows(s + '/w_ob', s + '/w_ob', x_rows, NH); vec(s + '/b_ob')
+                    rows(s + '/wx_hid', s + '/wx_hid', range(NH), 4 * NH)
+                rows(s + '/wh_hid', s + '/wh_hid', range(NH), 4 * NH); vec(s + '/b_hid')
+            if v == 'ma2c_dial':
+                for i in range(N):
+                    rows('dial/mfc_%d/w' % i, 'dial/mfc_%d/w' % i, range(NH), NH); vec('dial/mfc_%d/b' % i)
+            for i in range(N):
+                heads(i, '%s/pi_%d' % (sc, i), '%s/v_%d' % (sc, i))
         self._idx, self._tight = idx, tight
         self._tight_shapes = dict(tight)
         # `entries` is what callers enumerate (names, shapes, checkpoints): reference tensors; offset = first element
@@ -389,7 +441,7 @@ class HeteroLayout(ModelLayout):
         self.by_name = {n: (o, s) for n, o, s in self.entries}
 
     def creation_order(self):
-        return list(self._tight)          # built in tf.get_variable order (cells, [mfc], heads)
+        return list(self._tight)          # built in tf.get_variable order
 
     def pack(self, params):
         flat = np.zeros(self.n_param, dtype=np.float32)
