@@ -9,7 +9,7 @@ import os
 
 import torch
 
-MAX_AGENT, MAX_NBR, NH, MAX_NA = 32, 4, 64, 8
+MAX_AGENT, MAX_NBR, NH, MAX_NA = 128, 4, 64, 8
 IA2C, NC, IC3, DIAL = 0, 1, 2, 3
 SAMPLE_NONE, SAMPLE_UNIFORM, SAMPLE_PHILOX, SAMPLE_GREEDY = 0, 1, 2, 3
 CATCHUP, SLOWDOWN = 0, 1

@@ -397,6 +397,8 @@ __global__ void rng_advance_kernel(uint64_t* rng, uint64_t n) {
 }
 
 constexpr int FWD_BM = 64, FWD_TY = 16;
+NMARL_PARAMS_FIT(nmarl_model, FwdK);                                             // cell_fwd_kernel
+NMARL_PARAMS_FIT(nmarl_model, int, const float*, const float*, float*);          // dial_msg_kernel
 
 template <int VAR, int MODE>
 int launch_fwd(const nmarl_model* m, const FwdK& k, cudaStream_t st) {

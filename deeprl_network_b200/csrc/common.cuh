@@ -49,6 +49,21 @@ void nmarl_set_error(const char* fmt, ...);
     }                                                                                       \
   } while (0)
 
+// ---- transposed weight copies for the FFMA backward / DIAL message-gradient kernels (train.cu) ----------------------
+// One launch for all agents; `jobs` selects [wx;wh]^T -> t_wxh, w_msg^T -> t_w_msg, w_mfc^T -> t_mfc.
+enum { NMARL_TJ_WXH = 1, NMARL_TJ_MSG = 2, NMARL_TJ_MFC = 4 };
+int nmarl_launch_transposes(const nmarl_model* m, int jobs, const float* params, float* wt, cudaStream_t st);
+
+// ---- kernel-parameter budget ----------------------------------------------------------------------------------------
+// Kernels take the model descriptor (up to NMARL_MAX_AGENT agents) by value; sm_90 with CUDA >= 12.1 accepts at most
+// 32 764 bytes of parameters per launch.  Every such kernel states its parameter list here (the +16 per item covers
+// alignment padding between parameters).
+constexpr size_t NMARL_MAX_PARAM_BYTES = 32764;
+template <typename... Ts>
+constexpr size_t nmarl_param_bytes() { return (size_t(0) + ... + (sizeof(Ts) + 16)); }
+#define NMARL_PARAMS_FIT(...) \
+  static_assert(nmarl_param_bytes<__VA_ARGS__>() <= NMARL_MAX_PARAM_BYTES, "kernel parameters exceed 32 764 bytes")
+
 // ---- kernel launch with optional programmatic dependent launch (see tc.cuh: pdl_wait) ---------------------------
 // NMARL_NO_PDL=1 in the environment turns the attribute off (A/B switch; the device-side instructions become no-ops).
 bool nmarl_pdl_enabled();

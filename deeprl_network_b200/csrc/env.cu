@@ -2,7 +2,7 @@
 // Compiled with --fmad=false: the reference is NumPy float64 without FMA contraction, and the
 // kernels below keep its operation order so h, v, u and the rewards are bit-identical.
 //
-// Step kernel: one thread per (env, agent) -- see cacc_step_kernel.  Reset kernel: one thread per env (off the
+// Step kernel: one thread per env and agent row -- see cacc_step_kernel.  Reset kernel: one thread per env (off the
 // critical path).  All arrays are [agent][env], so a warp's loads/stores are coalesced over envs.
 //
 // Restates envs/cacc_env.py: step :191-242, reward :40-52, observation :54-65,
@@ -82,13 +82,16 @@ __global__ void cacc_reset_kernel(const EnvK k, const double* __restrict__ u01, 
   }
 }
 
-// One thread per (env, agent): blockDim = (32 envs, N agents), so a warp is one agent over 32 consecutive envs
-// (coalesced [agent][env] accesses) and the serial vehicle chain of the reference disappears: vehicle i's update
-// needs its predecessor's OLD and NEW speed, and the predecessor's new speed depends only on the predecessor's own
-// old state (and on ITS predecessor's old speed) -- each thread recomputes it with the very same operations, so
-// every number is bit-identical to the sequential sweep.  Reads of the old state, __syncthreads, then writes.
-// The per-env reductions (collision = min headway, global reward = np.sum over agents) run in shared memory in the
-// reference's order (sequential / 8 strided accumulators + pairwise tree, exactly what np.sum does).
+// Block = 32 envs x NY = min(N, 32) agent rows; a warp is one agent over 32 consecutive envs (coalesced [agent][env]
+// accesses) and thread row y handles agents y, y + NY, y + 2 NY, ... (at most ENV_J of them).  The serial vehicle chain
+// of the reference disappears: vehicle i's update needs its predecessor's OLD and NEW speed, and the predecessor's new
+// speed depends only on the predecessor's own old state (and on ITS predecessor's old speed) -- each thread recomputes
+// it with the very same operations, so every number is bit-identical to the sequential sweep.  Every old value of the
+// block's envs is read, __syncthreads, then the new state is written.
+// The per-env reductions run in shared memory: collision = min headway (per-thread minima, then a min over the rows:
+// min is exact in any order), global reward = np.sum over agents in the reference's order (sequential below 8 values,
+// otherwise 8 strided accumulators + pairwise tree + sequential tail: NumPy's pairwise-sum block, which is the whole
+// sum for N <= 128 = PW_BLOCKSIZE = NMARL_MAX_AGENT).
 struct VehStep { double vn, uc; };
 __device__ __forceinline__ VehStep veh_update(const nmarl_cacc_cfg& c, int a, double h, double v, double lead) {
   const double al = (a & 1) ? 0.5 : 0.0;          // a_map = [(0,0),(.5,0),(0,.5),(.5,.5)]  (:275)
@@ -102,32 +105,44 @@ __device__ __forceinline__ VehStep veh_update(const nmarl_cacc_cfg& c, int a, do
   return r;
 }
 
-__global__ void cacc_step_kernel(const EnvK k, int train_mode, const int32_t* __restrict__ action, double* hs,
-                                 double* vs, double* us, int32_t* t, int32_t* collision,
-                                 const double* __restrict__ v_init, float* obs, int obs_stride, double* reward,
-                                 double* greward, float* done) {
-  extern __shared__ double sm_env[];                 // [2][N][32]: per-agent reward, new headway
+constexpr int ENV_ROWS = 32;                           // agent rows per block
+constexpr int ENV_J = NMARL_MAX_AGENT / ENV_ROWS;      // agents per thread, at most
+static_assert(NMARL_MAX_AGENT <= 128, "the global reward restates np.sum's pairwise block, exact up to 128 values");
+static_assert(NMARL_MAX_AGENT % ENV_ROWS == 0, "agent rows");
+
+__global__ void __launch_bounds__(32 * ENV_ROWS) cacc_step_kernel(const EnvK k, int train_mode,
+                                                                 const int32_t* __restrict__ action, double* hs,
+                                                                 double* vs, double* us, int32_t* t, int32_t* collision,
+                                                                 const double* __restrict__ v_init, float* obs,
+                                                                 int obs_stride, double* reward, double* greward,
+                                                                 float* done) {
+  extern __shared__ double sm_env[];                 // [N][32] per-agent reward, then [NY][32] per-thread min headway
   // programmatic dependent launch: the CTAs may already be resident while the policy call that produces `action`
   // finishes; let the next policy call's CTAs start their prologue as well
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
   asm volatile("griddepcontrol.wait;" ::: "memory");
   const nmarl_cacc_cfg& c = k.c;
-  const int N = c.n_agent, L = c.platoon_len, B = k.B;
-  const int e = threadIdx.x, i = threadIdx.y;
+  const int N = c.n_agent, L = c.platoon_len, B = k.B, NY = blockDim.y;
+  const int e = threadIdx.x, y = threadIdx.y;
   const int b = blockIdx.x * 32 + e;
   const bool live = b < B;
   double* s_r = sm_env;
   double* s_h = sm_env + N * 32;
   __shared__ int s_col[32];
-  const int pos = i % L;
-  const size_t o = (size_t)i * B + b;
   int tcur = 0, col = 0;
-  double h = 0.0, v = 0.0, uo = 0.0, hn = 0.0, vn = 0.0, un = 0.0, lead_new = 0.0, vi0 = 0.0;
-  if (live) {
-    tcur = t[b]; col = collision[b];
-    h = hs[o]; v = vs[o]; uo = us[o];
-    vi0 = v_init[(size_t)(i / L) * B + b];
-    hn = h; vn = v; un = uo;
+  if (live) { tcur = t[b]; col = collision[b]; }
+  double hn[ENV_J], vn[ENV_J], un[ENV_J];            // new state (the old one after a collision)
+  double hmin = 1e300;
+#pragma unroll
+  for (int j = 0; j < ENV_J; ++j) {
+    hn[j] = vn[j] = un[j] = 0.0;
+    const int i = y + NY * j;
+    if (!live || i >= N) continue;
+    const int pos = i % L;
+    const size_t o = (size_t)i * B + b;
+    const double h = hs[o], v = vs[o], uo = us[o];
+    const double vi0 = v_init[(size_t)(i / L) * B + b];
+    hn[j] = h; vn[j] = v; un[j] = uo;
     if (!col) {
       double lead, lead_next;
       if (pos) {
@@ -141,33 +156,39 @@ __global__ void cacc_step_kernel(const EnvK k, int train_mode, const int32_t* __
         lead_next = leader_speed(c, vi0, tcur + 1);
       }
       const VehStep s = veh_update(c, action[o], h, v, lead);
-      vn = s.vn; un = s.uc;
-      hn = h + 0.5 * c.dt * (lead + lead_next - v - vn);
-      lead_new = lead_next;                          // leader's speed as the NEW observation sees it (pos > 0)
-      double r = -((hn - c.h_star) * (hn - c.h_star));
-      r = r + (-c.rew_a * ((vn - c.v_star) * (vn - c.v_star)));
-      r = r + (-c.rew_b * (un * un));
+      vn[j] = s.vn; un[j] = s.uc;
+      hn[j] = h + 0.5 * c.dt * (lead + lead_next - v - vn[j]);
+      double r = -((hn[j] - c.h_star) * (hn[j] - c.h_star));
+      r = r + (-c.rew_a * ((vn[j] - c.v_star) * (vn[j] - c.v_star)));
+      r = r + (-c.rew_b * (un[j] * un[j]));
       if (train_mode) {
-        const double m = fmin(hn - 10.0, 0.0);
+        const double m = fmin(hn[j] - 10.0, 0.0);
         r = r + (-5.0 * (m * m));
       } else {
         r = r + 0.0;
       }
       s_r[i * 32 + e] = r;
-      s_h[i * 32 + e] = hn;
-    } else if (pos) {
-      lead_new = vs[o - B];                          // frozen after a collision: the state does not move
+      hmin = fmin(hmin, hn[j]);
     }
   }
+  s_h[y * 32 + e] = hmin;
   __syncthreads();                                   // every old value has been read
-  if (live && !col) { hs[o] = hn; vs[o] = vn; us[o] = un; }
-  if (live && i == 0) {
+  if (live && !col) {
+#pragma unroll
+    for (int j = 0; j < ENV_J; ++j) {
+      const int i = y + NY * j;
+      if (i >= N) continue;
+      const size_t o = (size_t)i * B + b;
+      hs[o] = hn[j]; vs[o] = vn[j]; us[o] = un[j];
+    }
+  }
+  if (live && y == 0) {
     double gsum;
     int cnew = col;
     if (!col) {
-      double hmin = 1e300;
-      for (int j = 0; j < N; ++j) hmin = fmin(hmin, s_h[j * 32 + e]);
-      if (hmin < c.h_min) { cnew = 1; collision[b] = 1; }       // collision latch (:42-44)
+      double hm = 1e300;
+      for (int yy = 0; yy < NY; ++yy) hm = fmin(hm, s_h[yy * 32 + e]);
+      if (hm < c.h_min) { cnew = 1; collision[b] = 1; }         // collision latch (:42-44)
     }
     if (cnew) {
       gsum = -c.G * (double)N;                       // sum of N equal values is exact in any order
@@ -194,17 +215,25 @@ __global__ void cacc_step_kernel(const EnvK k, int train_mode, const int32_t* __
     const bool d = (cnew && (tn % c.batch_size == 0)) || (tn == c.T);
     done[b] = d ? 1.0f : 0.0f;
   }
-  __syncthreads();
+  __syncthreads();                                   // the new state of the block's envs is in hs / vs / us
   if (!live) return;
-  if (!c.global_reward) reward[o] = s_col[e] ? -c.G : s_r[i * 32 + e];     // frozen / new collision: -G (:193-194)
-  // observation from the NEW state and the NEW time (:54-65)
-  const double lead = pos ? lead_new : leader_speed(c, vi0, tcur + 1);
-  float* ob = obs + o * obs_stride;
-  ob[0] = (float)((vn - c.v_star) / c.v_star);
-  ob[1] = (float)clipd((lead - vn) / 5.0, -2.0, 2.0);
-  ob[2] = (float)clipd((ovm_vh(c, hn) - vn) / 5.0, -2.0, 2.0);
-  ob[3] = (float)((hn + (lead - vn) * c.dt - c.h_star) / c.h_star);
-  ob[4] = (float)(un / c.u_max);
+#pragma unroll
+  for (int j = 0; j < ENV_J; ++j) {
+    const int i = y + NY * j;
+    if (i >= N) continue;
+    const int pos = i % L;
+    const size_t o = (size_t)i * B + b;
+    if (!c.global_reward) reward[o] = s_col[e] ? -c.G : s_r[i * 32 + e];   // frozen / new collision: -G (:193-194)
+    // observation from the NEW state and the NEW time (:54-65); the predecessor's new speed is the value its thread
+    // stored (frozen after a collision: the old one), bit-identical to the lead_next this thread computed
+    const double lead = pos ? vs[o - B] : leader_speed(c, v_init[(size_t)(i / L) * B + b], tcur + 1);
+    float* ob = obs + o * obs_stride;
+    ob[0] = (float)((vn[j] - c.v_star) / c.v_star);
+    ob[1] = (float)clipd((lead - vn[j]) / 5.0, -2.0, 2.0);
+    ob[2] = (float)clipd((ovm_vh(c, hn[j]) - vn[j]) / 5.0, -2.0, 2.0);
+    ob[3] = (float)((hn[j] + (lead - vn[j]) * c.dt - c.h_star) / c.h_star);
+    ob[4] = (float)(un[j] / c.u_max);
+  }
 }
 
 }  // namespace
@@ -228,10 +257,12 @@ extern "C" int nmarl_cacc_step(const nmarl_cacc_cfg* cfg, int B, int train_mode,
                                int obs_stride, double* reward, double* greward, float* done, void* stream) {
   NMARL_CHECK(cfg && B > 0 && action, "cacc_step: bad arguments");
   NMARL_CHECK(cfg->platoon_len > 0 && cfg->n_agent % cfg->platoon_len == 0, "cacc_step: n_agent %% platoon_len != 0");
-  NMARL_CHECK(cfg->n_agent <= 32, "cacc_step: n_agent > 32");
+  NMARL_CHECK(cfg->n_agent > 0 && cfg->n_agent <= NMARL_MAX_AGENT, "cacc_step: n_agent %d out of range (1..%d)",
+              cfg->n_agent, NMARL_MAX_AGENT);
   EnvK k{*cfg, B};
-  const dim3 blk(32, cfg->n_agent);
-  const size_t smem = (size_t)2 * cfg->n_agent * 32 * sizeof(double);
+  const int rows = cfg->n_agent < ENV_ROWS ? cfg->n_agent : ENV_ROWS;
+  const dim3 blk(32, rows);
+  const size_t smem = (size_t)(cfg->n_agent + rows) * 32 * sizeof(double);     // <= 40 KB: no opt-in needed
   NMARL_CUDA(nmarl_launch(cacc_step_kernel, dim3((B + 31) / 32), blk, smem, (cudaStream_t)stream, true, k, train_mode,
                           action, hs, vs, us, t, collision, v_init, obs, obs_stride, reward, greward, done));
   NMARL_LAUNCH_CHECK();

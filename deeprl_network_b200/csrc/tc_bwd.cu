@@ -262,6 +262,8 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_cell_bwd_kernel(const __grid
   }
 }
 
+NMARL_PARAMS_FIT(nmarl_model, BwdK);                                             // tc_cell_bwd_kernel
+
 template <int VAR, bool FM, bool RAW>
 int launch_tc_bwd_fm(const nmarl_model* m, const BwdK& k, cudaStream_t st) {
   auto kern = tc_cell_bwd_kernel<VAR, FM, RAW>;

@@ -475,6 +475,8 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_cell_fwd_kernel(const __grid
 }
 
 
+NMARL_PARAMS_FIT(nmarl_model, FwdK);                                             // tc_cell_fwd_kernel
+
 template <int VAR, int MODE, bool FM>
 int launch_tc_fm(const nmarl_model* m, const FwdK& k, cudaStream_t st) {
   auto kern = tc_cell_fwd_kernel<VAR, MODE, FM>;
@@ -527,22 +529,6 @@ int nmarl_tc_launch_fwd(const nmarl_model* m, const FwdK& k, int mode, cudaStrea
 }
 
 namespace {
-__global__ void tc_transpose_kernel(const float* __restrict__ src, float* __restrict__ dst, int rows, int cols) {
-  __shared__ float tile[32][33];
-  const int c0 = blockIdx.x * 32, r0 = blockIdx.y * 32;
-  for (int y = threadIdx.y; y < 32; y += blockDim.y) {
-    const int r = r0 + y, cidx = c0 + threadIdx.x;
-    tile[y][threadIdx.x] = (r < rows && cidx < cols) ? src[(size_t)r * cols + cidx] : 0.f;
-  }
-  __syncthreads();
-  for (int y = threadIdx.y; y < 32; y += blockDim.y) {
-    const int cidx = c0 + y, r = r0 + threadIdx.x;
-    if (r < rows && cidx < cols) dst[(size_t)cidx * rows + r] = tile[threadIdx.x][y];
-  }
-}
-}  // namespace
-
-namespace {
 // One launch packs every tensor-core operand of every agent: per 32-deep k-block a [hi | lo] pair of 128B-swizzled
 // K-major tiles (see tc.cuh).  Job j of agent i (blockIdx.y = i * PACK_JOBS + j) is one matrix; the backward
 // operands (transposed weights) are gathered straight from the parameters with transposed indexing, so no
@@ -591,6 +577,7 @@ __global__ void __launch_bounds__(256) pack_all_kernel(const __grid_constant__ n
     *reinterpret_cast<float*>(tile + (size_t)p.N * 128 + off) = lo;
   }
 }
+NMARL_PARAMS_FIT(nmarl_model, const float*, float*);                             // pack_all_kernel
 }  // namespace
 
 extern "C" int nmarl_pack_weights(const nmarl_model* m, const float* params, float* wt, float* wpack, void* stream) {
@@ -598,15 +585,7 @@ extern "C" int nmarl_pack_weights(const nmarl_model* m, const float* params, flo
   cudaStream_t st = (cudaStream_t)stream;
   pack_all_kernel<<<dim3(16, m->n_agent * PACK_JOBS), 256, 0, st>>>(*m, params, wpack);
   NMARL_LAUNCH_CHECK();
-  if (m->variant == NMARL_DIAL) {          // DIAL's message-gradient kernel reads the plain transposed copies
-    dim3 blk(32, 8);
-    for (int i = 0; i < m->n_agent; ++i) {
-      const nmarl_agent& ag = m->agent[i];
-      const int Km = ag.n_nbr * NH;
-      if (Km > 0) tc_transpose_kernel<<<dim3(2, (Km + 31) / 32), blk, 0, st>>>(params + ag.o_w_msg, wt + ag.t_w_msg, Km, NH);
-      tc_transpose_kernel<<<dim3(2, 2), blk, 0, st>>>(params + ag.o_mfc_w, wt + ag.t_mfc, NH, NH);
-    }
-    NMARL_LAUNCH_CHECK();
-  }
+  // DIAL's message-gradient kernel reads the plain transposed copies (one launch for every agent)
+  if (m->variant == NMARL_DIAL && nmarl_launch_transposes(m, NMARL_TJ_MSG | NMARL_TJ_MFC, params, wt, st)) return 1;
   return 0;
 }

@@ -296,6 +296,10 @@ __global__ void __launch_bounds__(256) gate_bias_reduce_kernel(const __grid_cons
   }
 }
 
+NMARL_PARAMS_FIT(nmarl_model, TcWgK);                                            // tc_wgrad_kernel
+NMARL_PARAMS_FIT(nmarl_model, TcWgK, float*);                                    // tc_wgrad_reduce_kernel
+NMARL_PARAMS_FIT(nmarl_model, const float*, int, int, float*);                   // gate_bias_reduce_kernel
+
 int job_list(const nmarl_model* m, int* jobs) {
   int n = 0;
   jobs[n++] = J_GATE0;

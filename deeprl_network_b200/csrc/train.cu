@@ -67,18 +67,35 @@ __global__ void nstep_return_kernel(const RetK k, const double* __restrict__ rew
 }
 
 // ============================ transposes =======================================================
-__global__ void transpose_kernel(const float* __restrict__ src, float* __restrict__ dst, int rows, int cols) {
-  // dst[c][r] = src[r][c]; small matrices, 32x32 smem tiles
+// dst[c][r] = src[r][c] for every agent's selected weights in one launch: blockIdx.z = matrix (wx;wh / w_msg / w_mfc),
+// blockIdx.y = agent, blockIdx.x strides over the 32x32 smem tiles of that matrix.  Copies are exact, so the tiling
+// does not change a bit.
+constexpr int TRANSPOSE_CTAS = 64;            // [wx;wh] of NeurComm: 256 x 256 = 64 tiles
+__global__ void __launch_bounds__(256) transpose_all_kernel(const __grid_constant__ nmarl_model m, int jobs,
+                                                            const float* __restrict__ params, float* __restrict__ wt) {
   __shared__ float tile[32][33];
-  const int c0 = blockIdx.x * 32, r0 = blockIdx.y * 32;
-  for (int y = threadIdx.y; y < 32; y += blockDim.y) {
-    const int r = r0 + y, c = c0 + threadIdx.x;
-    tile[y][threadIdx.x] = (r < rows && c < cols) ? src[(size_t)r * cols + c] : 0.f;
-  }
-  __syncthreads();
-  for (int y = threadIdx.y; y < 32; y += blockDim.y) {
-    const int c = c0 + y, r = r0 + threadIdx.x;
-    if (r < rows && c < cols) dst[(size_t)c * rows + r] = tile[threadIdx.x][y];
+  const int j = blockIdx.z, i = blockIdx.y;
+  if (!(jobs & (1 << j))) return;
+  const nmarl_agent& ag = m.agent[i];
+  int rows = 0, cols = NH, src_off = 0, dst_off = 0;
+  if (j == 0) { rows = m.s_dim + NH; cols = NG; src_off = ag.o_wxh; dst_off = ag.t_wxh; }
+  else if (j == 1) { rows = (m.variant == NMARL_IC3) ? NH : ag.n_nbr * NH; src_off = ag.o_w_msg; dst_off = ag.t_w_msg; }
+  else { rows = NH; src_off = ag.o_mfc_w; dst_off = ag.t_mfc; }
+  const float* __restrict__ src = params + src_off;
+  float* __restrict__ dst = wt + dst_off;
+  const int tx = (cols + 31) / 32, ntile = tx * ((rows + 31) / 32);
+  for (int tl = blockIdx.x; tl < ntile; tl += gridDim.x) {
+    const int c0 = (tl % tx) * 32, r0 = (tl / tx) * 32;
+    __syncthreads();                          // the previous tile has been read out
+    for (int y = threadIdx.y; y < 32; y += blockDim.y) {
+      const int r = r0 + y, c = c0 + threadIdx.x;
+      tile[y][threadIdx.x] = (r < rows && c < cols) ? src[(size_t)r * cols + c] : 0.f;
+    }
+    __syncthreads();
+    for (int y = threadIdx.y; y < 32; y += blockDim.y) {
+      const int c = c0 + y, r = r0 + threadIdx.x;
+      if (r < rows && c < cols) dst[(size_t)c * rows + r] = tile[threadIdx.x][y];
+    }
   }
 }
 
@@ -818,7 +835,26 @@ int check_bwd_args(const nmarl_model* m, const nmarl_bwd_args* a) {
   return 0;
 }
 
+// parameter lists of the kernels above (the by-value descriptor and the per-agent arrays grow with NMARL_MAX_AGENT)
+NMARL_PARAMS_FIT(nmarl_model, BwdK);                                                             // cell_bwd_kernel
+NMARL_PARAMS_FIT(nmarl_model, int, const float*, const float*, const float*, float*, float*);    // dial_msg_bwd_kernel
+NMARL_PARAMS_FIT(nmarl_model, int, const float*, float*);                                        // transpose_all_kernel
+NMARL_PARAMS_FIT(WgK);
+NMARL_PARAMS_FIT(WgRedK);
+NMARL_PARAMS_FIT(nmarl_model, HeadK);
+NMARL_PARAMS_FIT(nmarl_model, HeadRedK);
+NMARL_PARAMS_FIT(OptK, float*, const float*, float*, const float*, const float*, float*);        // rmsprop_kernel
+NMARL_PARAMS_FIT(nmarl_model, HeadFwdK);
+NMARL_PARAMS_FIT(nmarl_model, const float*, float*, int);                                        // consensus kernels
+
 }  // namespace
+
+int nmarl_launch_transposes(const nmarl_model* m, int jobs, const float* params, float* wt, cudaStream_t st) {
+  if (jobs == 0) return 0;
+  transpose_all_kernel<<<dim3(TRANSPOSE_CTAS, m->n_agent, 3), dim3(32, 8), 0, st>>>(*m, jobs, params, wt);
+  NMARL_LAUNCH_CHECK();
+  return 0;
+}
 
 extern "C" int nmarl_loss_tiles(const nmarl_model* m, int B) { (void)m; return nmarl_fwd_tiles(B); }
 
@@ -907,23 +943,12 @@ extern "C" int nmarl_a2c_bptt(const nmarl_model* m, const nmarl_bwd_args* a, voi
   NMARL_CUDA(cudaMemsetAsync(a->grads, 0, (size_t)m->n_param * sizeof(float), st));
   // 1. transposed weights for the FFMA backward kernels and DIAL's message-gradient kernel (the tensor-core cell
   //    kernels read their own packed transposed operands, refreshed by nmarl_pack_weights)
+  //    One launch covers every agent.
   const bool tc_path = (a->wpack != nullptr && B % 128 == 0 && m->kx_pad <= 32 && m->kp_pad <= 32);
-  if (!tc_path || m->variant == NMARL_DIAL)
-  for (int i = 0; i < N; ++i) {
-    const nmarl_agent& ag = m->agent[i];
-    dim3 blk(32, 8);
-    {
-      const int rows = SD + NH, cols = NG;
-      transpose_kernel<<<dim3((cols + 31) / 32, (rows + 31) / 32), blk, 0, st>>>(a->params + ag.o_wxh, a->wt + ag.t_wxh, rows, cols);
-    }
-    if (m->variant != NMARL_IA2C) {
-      const int rows = (m->variant == NMARL_IC3) ? NH : ag.n_nbr * NH, cols = NH;
-      if (rows > 0) transpose_kernel<<<dim3((cols + 31) / 32, (rows + 31) / 32), blk, 0, st>>>(a->params + ag.o_w_msg, a->wt + ag.t_w_msg, rows, cols);
-    }
-    if (m->variant == NMARL_DIAL)
-      transpose_kernel<<<dim3(2, 2), blk, 0, st>>>(a->params + ag.o_mfc_w, a->wt + ag.t_mfc, NH, NH);
+  if (!tc_path || m->variant == NMARL_DIAL) {
+    const int jobs = NMARL_TJ_WXH | (m->variant != NMARL_IA2C ? NMARL_TJ_MSG : 0) | (m->variant == NMARL_DIAL ? NMARL_TJ_MFC : 0);
+    if (nmarl_launch_transposes(m, jobs, a->params, a->wt, st)) return 1;
   }
-  NMARL_LAUNCH_CHECK();
   // 1b. policy/value head weight gradients need only sv_dlv and h_seq: they run on a forked stream
   //     beside the BPTT chain (whose 256-CTA launches leave SMs idle in their second wave) and join
   //     before the weight-gradient phase, which shares the workspace.
@@ -1066,7 +1091,8 @@ extern "C" int nmarl_clip_rmsprop_step(const nmarl_model* m, float* params, floa
   } else {
     k.n_groups = 1; k.g_begin[0] = 0; k.g_end[0] = m->n_param;
   }
-  k.nblk = (k.n_groups == 1) ? 256 : 32;       // n_groups * nblk <= 1024 scratch floats
+  // n_groups * nblk <= 1024 scratch floats: 32 blocks per agent up to 32 agents, fewer beyond (8 at 128 agents)
+  k.nblk = (k.n_groups == 1) ? 256 : (k.n_groups <= 32 ? 32 : 1024 / k.n_groups);
   cudaStream_t st = (cudaStream_t)stream;
   sumsq_kernel<<<dim3(k.nblk, k.n_groups), 256, 0, st>>>(k, grads, scratch);
   NMARL_LAUNCH_CHECK();

@@ -27,7 +27,10 @@ extern "C" {
 #endif
 #pragma GCC visibility push(default)
 
-#define NMARL_MAX_AGENT 32
+/* 128: the env kernel's global reward reproduces np.sum bit for bit, whose 8-accumulator block covers at most
+ * 128 values (NumPy's PW_BLOCKSIZE), and the model descriptor kernels take by value, 48 + 128 x 192 = 24 624 bytes,
+ * stays inside the 32 764-byte kernel-parameter limit of sm_90 with room for each kernel's argument block       */
+#define NMARL_MAX_AGENT 128
 #define NMARL_MAX_NBR   4
 #define NMARL_NH        64      /* LSTM width (num_lstm = num_fc = 64 in every shipped config) */
 #define NMARL_MAX_NA    8
