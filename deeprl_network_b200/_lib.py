@@ -9,7 +9,8 @@ import os
 
 import torch
 
-MAX_AGENT, MAX_NBR, NH, MAX_NA = 128, 4, 64, 8
+MAX_AGENT, MAX_NBR, NH, MAX_NA = 128, 4, 64, 8       # NH: the width of the tensor-core kernels
+WIDTHS = (16, 32, 64)                                  # LSTM widths (num_lstm) the FFMA kernels run
 IA2C, NC, IC3, DIAL = 0, 1, 2, 3
 SAMPLE_NONE, SAMPLE_UNIFORM, SAMPLE_PHILOX, SAMPLE_GREEDY = 0, 1, 2, 3
 CATCHUP, SLOWDOWN = 0, 1

@@ -18,16 +18,13 @@ import torch
 
 from .. import _lib as L
 
-NH = L.NH
-
-
 class PolicyEngine:
     def __init__(self, layout, n_env, n_step, hp, flat_params=None, device=None, rng_seed=0,
                  distance_mask=None, coop_gamma=-1.0, group=None, use_tc=None):
         """hp: dict(v_coef, e_coef, max_grad_norm, alpha, epsilon, gamma, reward_norm, reward_clip)."""
         L.require_cuda()
         self.layout, self.B, self.T, self.hp = layout, int(n_env), int(n_step), dict(hp)
-        self.N, self.n_a = layout.N, layout.n_a
+        self.N, self.n_a, self.n_h = layout.N, layout.n_a, layout.n_h
         self.device = torch.device(device if device is not None else 'cuda:%d' % torch.cuda.current_device())
         self.group = group
         self.world = torch.distributed.get_world_size(group) if (group is not None or (
@@ -48,13 +45,16 @@ class PolicyEngine:
         # tensor-core path: packed 3xTF32 operands; used by the kernels when B % 128 == 0
         if use_tc is None:
             use_tc = os.environ.get('NMARL_NO_TC', '0') != '1'
-        # same conditions as nmarl_tc_fwd_supported / the bptt dispatch (csrc): whole 128-env tiles, narrow encoders
-        self.use_tc = bool(use_tc) and (self.B % 128 == 0) and layout.kx_pad <= 32 and layout.kp_pad <= 32
+        # same conditions as nmarl_tc_fwd_supported / the bptt dispatch (csrc): whole 128-env tiles, narrow encoders and
+        # the width the tensor-core kernels are built for; other widths run the FP32-FFMA kernels
+        self.use_tc = (bool(use_tc) and (self.B % 128 == 0) and layout.kx_pad <= 32 and layout.kp_pad <= 32
+                       and layout.n_h == L.NH)
         self.wpack = torch.zeros(layout.n_wp, **f32) if self.use_tc else None
         self.tc_err = torch.zeros(1, dtype=torch.int32, device=dev)
         # tensor-core path: LSTM state (and its gradients) feature-major [N,64,B] so that lane == env accesses are
         # coalesced; DIAL keeps env-major state (its message kernels are env-major)
         self.state_fm = self.use_tc and self.variant != 'ma2c_dial' and os.environ.get('NMARL_NO_STATE_FM', '0') != '1'
+        NH = self.n_h
         self._sshape = (N, NH, B) if self.state_fm else (N, B, NH)
         self.c = [torch.zeros(*self._sshape, **f32) for _ in range(2)]
         self.h = [torch.zeros(*self._sshape, **f32) for _ in range(2)]
@@ -155,14 +155,14 @@ class PolicyEngine:
             self.cur = 0
 
     def get_states_fw(self):
-        """[N, B, 128] = [c | h] like the reference's states_fw (env-major view whatever the device layout)."""
+        """[N, B, 2 * n_h] = [c | h] like the reference's states_fw (env-major view whatever the device layout)."""
         c, h = self.c[self.cur], self.h[self.cur]
         if self.state_fm:
             c, h = c.permute(0, 2, 1), h.permute(0, 2, 1)
         return torch.cat([c, h], dim=-1).contiguous()
 
     def set_states(self, c, h, bw=True):
-        """c, h: env-major [N, B, 64]."""
+        """c, h: env-major [N, B, n_h]."""
         if self.state_fm:
             c, h = c.permute(0, 2, 1), h.permute(0, 2, 1)
         self.c[self.cur].copy_(c); self.h[self.cur].copy_(h)
@@ -330,7 +330,7 @@ class PolicyEngine:
     def _alloc_train(self):
         if self._train_ready:
             return
-        lay, N, B, T, dev = self.layout, self.N, self.B, self.T, self.device
+        lay, N, B, T, dev, NH = self.layout, self.N, self.B, self.T, self.device, self.n_h
         f32 = dict(dtype=torch.float32, device=dev)
         z = lambda *s: torch.zeros(*s, **f32)
         self.h_seq, self.c_seq = z(T + 2, *self._sshape), z(T + 2, *self._sshape)       # +1 slot for the bootstrap p-call
@@ -338,14 +338,14 @@ class PolicyEngine:
         self.sv_xin = z(T, N, B, lay.ld_in)
         self.sv_sh = z(T, N, B, lay.s_dim + NH)
         self.sv_gates = z(T, N, B, 4 * NH)
-        self.sv_enc = z(T, N, B, 128) if self.variant in ('ma2c_ic3', 'ma2c_dial') else None
+        self.sv_enc = z(T, N, B, 2 * NH) if self.variant in ('ma2c_ic3', 'ma2c_dial') else None
         self.sv_dlv = z(T, N, B, 8)
         # tensor-core path: sv_dz holds per-tile gate-bias partial sums, sv_dpre is unused (operand tiles instead)
         self.sv_dz = z(T, N, B // 32, 4 * NH) if self.use_tc else z(T, N, B, 4 * NH)
-        self.sv_dpre = z(4) if self.use_tc else z(T, N, B, 192)
+        self.sv_dpre = z(4) if self.use_tc else z(T, N, B, 3 * NH)
         # tensor-core path: dz / encoder pre-activation gradients additionally as K-major [hi | lo] operand tiles
-        ndp = {'ma2c_nc': 192, 'ia2c': 64}.get(self.variant, 128)
-        self.sv_dzT = z(T, N, B // 32, 2 * 256 * 32) if self.use_tc else None
+        ndp = {'ma2c_nc': 3 * NH, 'ia2c': NH}.get(self.variant, 2 * NH)
+        self.sv_dzT = z(T, N, B // 32, 2 * 4 * NH * 32) if self.use_tc else None
         self.sv_dpT = z(T, N, B // 32, 2 * ndp * 32) if self.use_tc else None
         self.sv_dmp = z(T, N, B, NH) if self.variant == 'ma2c_dial' else None
         self.dh_rec, self.dc_rec = z(2, *self._sshape), z(2, *self._sshape)
@@ -418,6 +418,7 @@ class PolicyEngine:
         self.launches += 2
         if self.agent_name == 'ma2c_cu':     # ConsensusPolicy.backward: sess.run(_consensus_update) after the optimizer
             if getattr(self, '_cu_scratch', None) is None:
+                NH = self.n_h
                 self._cu_scratch = torch.zeros(self.N * ((self.layout.s_dim + NH) * 4 * NH + 4 * NH),
                                                dtype=torch.float32, device=self.device)
             L.check(L.lib().nmarl_consensus_update(C.byref(self.model), L.ptr(self.params), L.ptr(self._cu_scratch),

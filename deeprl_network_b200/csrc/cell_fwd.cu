@@ -15,23 +15,23 @@
 
 namespace {
 
-template <int BM, int KC>
+template <int BM, int KC, int H>
 __host__ __device__ inline size_t fwd_region0_floats(const nmarl_model& m) {
   const size_t in = (size_t)BM * (m.kx_pad + m.kp_pad + m.km_pad);
-  const size_t ring = (size_t)2 * KC * NG;
-  const size_t hs = (size_t)BM * (NH + 4);
+  const size_t ring = (size_t)2 * KC * (4 * H);
+  const size_t hs = (size_t)BM * (H + 4);
   size_t r = in > ring ? in : ring;
   return r > hs ? r : hs;
 }
-template <int BM, int KC>
+template <int BM, int KC, int H>
 __host__ __device__ inline size_t fwd_smem_floats(const nmarl_model& m) {
-  return fwd_region0_floats<BM, KC>(m) + (size_t)BM * (m.s_dim + NH + 4) + (size_t)2 * KC * NH;
+  return fwd_region0_floats<BM, KC, H>(m) + (size_t)BM * (m.s_dim + H + 4) + (size_t)2 * KC * H;
 }
 
-template <int VAR, int MODE, int BM, int TY>
-__global__ void __launch_bounds__(16 * TY) cell_fwd_kernel(const __grid_constant__ nmarl_model m,
+template <int VAR, int MODE, int BM, int TY, int H>
+__global__ void __launch_bounds__(H / 4 * TY) cell_fwd_kernel(const __grid_constant__ nmarl_model m,
                                                           const __grid_constant__ FwdK k) {
-  constexpr int NT = 16 * TY, TM = BM / TY, KC = 16;
+  constexpr int NT = H / 4 * TY, TM = BM / TY, KC = 16;
   static_assert(BM % TY == 0 && NT >= BM, "tile/thread mismatch");
   extern __shared__ __align__(16) float smem[];
   const nmarl_fwd_args& a = k.a;
@@ -39,16 +39,16 @@ __global__ void __launch_bounds__(16 * TY) cell_fwd_kernel(const __grid_constant
   const nmarl_agent& ag = m.agent[i];
   const int B = a.B, b0 = blockIdx.x * BM;
   const int rows = min(BM, B - b0);
-  const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
+  const int tid = threadIdx.x, tx = tid & (H / 4 - 1), ty = tid >> nmarl_log2(H / 4);
   const int n_a = m.n_a, SD = m.s_dim;
   const int LDI = m.kx_pad + m.kp_pad + m.km_pad, PO = m.kx_pad, MO = m.kx_pad + m.kp_pad;
-  const int LDS = SD + NH + 4;
+  const int LDS = SD + H + 4;
   float* IN = smem;
-  float* SH = smem + fwd_region0_floats<BM, KC>(m);
+  float* SH = smem + fwd_region0_floats<BM, KC, H>(m);
   float* WsE = SH + (size_t)BM * LDS;
   float* WsG = smem;                     // gate-weight ring aliases IN (dead after the encoders)
   float* Hs = smem;                      // new-h tile aliases the ring (dead after the gate GEMM)
-  constexpr int LDH = NH + 4;
+  constexpr int LDH = H + 4;
   const float* __restrict__ P = a.params;
 
   // ---- phase 0: gather inputs (agent-major global -> row-major smem) ------------------------
@@ -79,20 +79,20 @@ __global__ void __launch_bounds__(16 * TY) cell_fwd_kernel(const __grid_constant
     const int q4 = m.km_pad / 4;
     for (int idx = tid; idx < BM * q4; idx += NT) {
       const int r = idx / q4, c4 = idx - r * q4;
-      const int s = c4 / (NH / 4), u4 = c4 - s * (NH / 4);
+      const int s = c4 / (H / 4), u4 = c4 - s * (H / 4);
       float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
       if (r < rows && s < ag.n_nbr)
-        v = *reinterpret_cast<const float4*>(src + ((size_t)ag.nbr[s] * B + b0 + r) * NH + 4 * u4);
+        v = *reinterpret_cast<const float4*>(src + ((size_t)ag.nbr[s] * B + b0 + r) * H + 4 * u4);
       *reinterpret_cast<float4*>(IN + r * LDI + MO + 4 * c4) = v;
     }
   }
   if (VAR == NMARL_IC3) {                                             // mean of neighbours' h (utils.py:395)
-    for (int idx = tid; idx < BM * (NH / 4); idx += NT) {
-      const int r = idx / (NH / 4), u4 = idx - r * (NH / 4);
+    for (int idx = tid; idx < BM * (H / 4); idx += NT) {
+      const int r = idx / (H / 4), u4 = idx - r * (H / 4);
       float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
       if (r < rows) {
         for (int s = 0; s < ag.n_nbr; ++s) {
-          const float4 w = *reinterpret_cast<const float4*>(a.h_in + ((size_t)ag.nbr[s] * B + b0 + r) * NH + 4 * u4);
+          const float4 w = *reinterpret_cast<const float4*>(a.h_in + ((size_t)ag.nbr[s] * B + b0 + r) * H + 4 * u4);
           v.x += w.x; v.y += w.y; v.z += w.z; v.w += w.w;
         }
         const float nn = (float)ag.n_nbr;
@@ -101,11 +101,11 @@ __global__ void __launch_bounds__(16 * TY) cell_fwd_kernel(const __grid_constant
       *reinterpret_cast<float4*>(IN + r * LDI + MO + 4 * u4) = v;
     }
   }
-  for (int idx = tid; idx < BM * (NH / 4); idx += NT) {                // own h, done-masked (utils.py:189-190)
-    const int r = idx / (NH / 4), u4 = idx - r * (NH / 4);
+  for (int idx = tid; idx < BM * (H / 4); idx += NT) {                // own h, done-masked (utils.py:189-190)
+    const int r = idx / (H / 4), u4 = idx - r * (H / 4);
     float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
     if (r < rows) {
-      v = *reinterpret_cast<const float4*>(a.h_in + ((size_t)i * B + b0 + r) * NH + 4 * u4);
+      v = *reinterpret_cast<const float4*>(a.h_in + ((size_t)i * B + b0 + r) * H + 4 * u4);
       const float nd = 1.0f - a.done[b0 + r];
       v.x *= nd; v.y *= nd; v.z *= nd; v.w *= nd;
     }
@@ -127,7 +127,7 @@ __global__ void __launch_bounds__(16 * TY) cell_fwd_kernel(const __grid_constant
     float acc[TM][4];
 #pragma unroll
     for (int q = 0; q < TM; ++q) { acc[q][0] = acc[q][1] = acc[q][2] = acc[q][3] = 0.f; }
-    gemm_rowA<TM, 1, TY, KC>(acc, IN, LDI, Kx, P + ag.o_w_ob, NH, WsE, tid);
+    gemm_rowA<TM, 1, TY, KC, H>(acc, IN, LDI, Kx, P + ag.o_w_ob, H, WsE, tid);
     const float4 bb = *reinterpret_cast<const float4*>(P + ag.o_b_ob + 4 * tx);
 #pragma unroll
     for (int q = 0; q < TM; ++q) {
@@ -138,7 +138,7 @@ __global__ void __launch_bounds__(16 * TY) cell_fwd_kernel(const __grid_constant
       if (VAR == NMARL_NC || VAR == NMARL_IA2C)
         *reinterpret_cast<float4*>(SH + r * LDS + 4 * tx) = make_float4(sv[q][0], sv[q][1], sv[q][2], sv[q][3]);
       if (MODE == MODE_TRAIN && (VAR == NMARL_IC3 || VAR == NMARL_DIAL) && r < rows)
-        *reinterpret_cast<float4*>(k.sv_enc + ((size_t)i * B + b0 + r) * 128 + 4 * tx) =
+        *reinterpret_cast<float4*>(k.sv_enc + ((size_t)i * B + b0 + r) * (2 * H) + 4 * tx) =
             make_float4(sv[q][0], sv[q][1], sv[q][2], sv[q][3]);
     }
   }
@@ -146,12 +146,12 @@ __global__ void __launch_bounds__(16 * TY) cell_fwd_kernel(const __grid_constant
     float acc[TM][4];
 #pragma unroll
     for (int q = 0; q < TM; ++q) { acc[q][0] = acc[q][1] = acc[q][2] = acc[q][3] = 0.f; }
-    gemm_rowA<TM, 1, TY, KC>(acc, IN + PO, LDI, ag.n_nbr * n_a, P + ag.o_w_fp, NH, WsE, tid);
+    gemm_rowA<TM, 1, TY, KC, H>(acc, IN + PO, LDI, ag.n_nbr * n_a, P + ag.o_w_fp, H, WsE, tid);
     const float4 bb = *reinterpret_cast<const float4*>(P + ag.o_b_fp + 4 * tx);
 #pragma unroll
     for (int q = 0; q < TM; ++q) {
       const int r = ty + TY * q;
-      *reinterpret_cast<float4*>(SH + r * LDS + NH + 4 * tx) =
+      *reinterpret_cast<float4*>(SH + r * LDS + H + 4 * tx) =
           make_float4(fmaxf(acc[q][0] + bb.x, 0.f), fmaxf(acc[q][1] + bb.y, 0.f), fmaxf(acc[q][2] + bb.z, 0.f),
                       fmaxf(acc[q][3] + bb.w, 0.f));
     }
@@ -160,8 +160,8 @@ __global__ void __launch_bounds__(16 * TY) cell_fwd_kernel(const __grid_constant
     float acc[TM][4];
 #pragma unroll
     for (int q = 0; q < TM; ++q) { acc[q][0] = acc[q][1] = acc[q][2] = acc[q][3] = 0.f; }
-    const int Km = (VAR == NMARL_IC3) ? NH : ag.n_nbr * NH;
-    gemm_rowA<TM, 1, TY, KC>(acc, IN + MO, LDI, Km, P + ag.o_w_msg, NH, WsE, tid);
+    const int Km = (VAR == NMARL_IC3) ? H : ag.n_nbr * H;
+    gemm_rowA<TM, 1, TY, KC, H>(acc, IN + MO, LDI, Km, P + ag.o_w_msg, H, WsE, tid);
     // DIAL without a message encoder (o_b_msg < 0, see nmarl.h): relu(0 + 0) = 0 and no own-action one-hot below
     const bool has_msg = ag.o_b_msg >= 0;
     const float4 bb = has_msg ? *reinterpret_cast<const float4*>(P + ag.o_b_msg + 4 * tx) : make_float4(0.f, 0.f, 0.f, 0.f);
@@ -170,7 +170,7 @@ __global__ void __launch_bounds__(16 * TY) cell_fwd_kernel(const __grid_constant
       const int r = ty + TY * q;
       float z[4] = {acc[q][0] + bb.x, acc[q][1] + bb.y, acc[q][2] + bb.z, acc[q][3] + bb.w};
       if (VAR == NMARL_NC) {
-        *reinterpret_cast<float4*>(SH + r * LDS + 2 * NH + 4 * tx) =
+        *reinterpret_cast<float4*>(SH + r * LDS + 2 * H + 4 * tx) =
             make_float4(fmaxf(z[0], 0.f), fmaxf(z[1], 0.f), fmaxf(z[2], 0.f), fmaxf(z[3], 0.f));
       } else if (VAR == NMARL_IC3) {                                    // s = tanh(..) + m W_msg + b  (utils.py:400)
         *reinterpret_cast<float4*>(SH + r * LDS + 4 * tx) =
@@ -188,7 +188,7 @@ __global__ void __launch_bounds__(16 * TY) cell_fwd_kernel(const __grid_constant
         for (int j = 0; j < 4; ++j) o[j] = (sv[q][j] + hm[j]) + ((4 * tx + j) == am ? 1.0f : 0.0f);
         *reinterpret_cast<float4*>(SH + r * LDS + 4 * tx) = make_float4(o[0], o[1], o[2], o[3]);
         if (MODE == MODE_TRAIN && r < rows)
-          *reinterpret_cast<float4*>(k.sv_enc + ((size_t)i * B + b0 + r) * 128 + NH + 4 * tx) =
+          *reinterpret_cast<float4*>(k.sv_enc + ((size_t)i * B + b0 + r) * (2 * H) + H + 4 * tx) =
               make_float4(hm[0], hm[1], hm[2], hm[3]);
       }
     }
@@ -201,19 +201,19 @@ __global__ void __launch_bounds__(16 * TY) cell_fwd_kernel(const __grid_constant
   for (int q = 0; q < TM; ++q)
 #pragma unroll
     for (int c = 0; c < 16; ++c) acc[q][c] = 0.f;
-  gemm_rowA<TM, 4, TY, KC>(acc, SH, LDS, SD + NH, P + ag.o_wxh, NG, WsG, tid);
+  gemm_rowA<TM, 4, TY, KC, H>(acc, SH, LDS, SD + H, P + ag.o_wxh, (4 * H), WsG, tid);
   if (MODE == MODE_TRAIN) {                                             // save [s | h^] for wgrad
-    const int q4 = (SD + NH) / 4;
+    const int q4 = (SD + H) / 4;
     for (int idx = tid; idx < rows * q4; idx += NT) {
       const int r = idx / q4, c4 = idx - r * q4;
-      *reinterpret_cast<float4*>(k.sv_sh + ((size_t)i * B + b0 + r) * (SD + NH) + 4 * c4) =
+      *reinterpret_cast<float4*>(k.sv_sh + ((size_t)i * B + b0 + r) * (SD + H) + 4 * c4) =
           *reinterpret_cast<const float4*>(SH + r * LDS + 4 * c4);
     }
   }
   {
     float4 bg[4];
 #pragma unroll
-    for (int g = 0; g < 4; ++g) bg[g] = *reinterpret_cast<const float4*>(P + ag.o_b + g * NH + 4 * tx);
+    for (int g = 0; g < 4; ++g) bg[g] = *reinterpret_cast<const float4*>(P + ag.o_b + g * H + 4 * tx);
 #pragma unroll
     for (int q = 0; q < TM; ++q) {
       const int r = ty + TY * q;
@@ -221,7 +221,7 @@ __global__ void __launch_bounds__(16 * TY) cell_fwd_kernel(const __grid_constant
       if (r < rows) {
         const size_t row = (size_t)i * B + b0 + r;
         const float nd = 1.0f - a.done[b0 + r];
-        const float4 cp4 = *reinterpret_cast<const float4*>(a.c_in + row * NH + 4 * tx);
+        const float4 cp4 = *reinterpret_cast<const float4*>(a.c_in + row * H + 4 * tx);
         const float cp[4] = {cp4.x * nd, cp4.y * nd, cp4.z * nd, cp4.w * nd};
         float cn[4], gi[4], gf[4], go[4], gu[4];
 #pragma unroll
@@ -234,15 +234,15 @@ __global__ void __launch_bounds__(16 * TY) cell_fwd_kernel(const __grid_constant
           hn[j] = go[j] * tanhf(cn[j]);
         }
         if (MODE != MODE_V) {
-          *reinterpret_cast<float4*>(a.c_out + row * NH + 4 * tx) = make_float4(cn[0], cn[1], cn[2], cn[3]);
-          *reinterpret_cast<float4*>(a.h_out + row * NH + 4 * tx) = make_float4(hn[0], hn[1], hn[2], hn[3]);
+          *reinterpret_cast<float4*>(a.c_out + row * H + 4 * tx) = make_float4(cn[0], cn[1], cn[2], cn[3]);
+          *reinterpret_cast<float4*>(a.h_out + row * H + 4 * tx) = make_float4(hn[0], hn[1], hn[2], hn[3]);
         }
         if (MODE == MODE_TRAIN) {
-          float* gs = k.sv_gates + row * NG + 4 * tx;
-          *reinterpret_cast<float4*>(gs + 0 * NH) = make_float4(gi[0], gi[1], gi[2], gi[3]);
-          *reinterpret_cast<float4*>(gs + 1 * NH) = make_float4(gf[0], gf[1], gf[2], gf[3]);
-          *reinterpret_cast<float4*>(gs + 2 * NH) = make_float4(go[0], go[1], go[2], go[3]);
-          *reinterpret_cast<float4*>(gs + 3 * NH) = make_float4(gu[0], gu[1], gu[2], gu[3]);
+          float* gs = k.sv_gates + row * (4 * H) + 4 * tx;
+          *reinterpret_cast<float4*>(gs + 0 * H) = make_float4(gi[0], gi[1], gi[2], gi[3]);
+          *reinterpret_cast<float4*>(gs + 1 * H) = make_float4(gf[0], gf[1], gf[2], gf[3]);
+          *reinterpret_cast<float4*>(gs + 2 * H) = make_float4(go[0], go[1], go[2], go[3]);
+          *reinterpret_cast<float4*>(gs + 3 * H) = make_float4(gu[0], gu[1], gu[2], gu[3]);
         }
       }
       *reinterpret_cast<float4*>(Hs + r * LDH + 4 * tx) = make_float4(hn[0], hn[1], hn[2], hn[3]);
@@ -255,9 +255,9 @@ __global__ void __launch_bounds__(16 * TY) cell_fwd_kernel(const __grid_constant
   if (tid < rows) {
     const int r = tid, b = b0 + r;
     const size_t row = (size_t)i * B + b;
-    float h[NH];
+    float h[H];
 #pragma unroll
-    for (int u4 = 0; u4 < NH / 4; ++u4) {
+    for (int u4 = 0; u4 < H / 4; ++u4) {
       const float4 t4 = *reinterpret_cast<const float4*>(Hs + r * LDH + 4 * u4);
       h[4 * u4] = t4.x; h[4 * u4 + 1] = t4.y; h[4 * u4 + 2] = t4.z; h[4 * u4 + 3] = t4.w;
     }
@@ -267,7 +267,7 @@ __global__ void __launch_bounds__(16 * TY) cell_fwd_kernel(const __grid_constant
       for (int c = 0; c < n_a; ++c) {
         float l = 0.f;
 #pragma unroll
-        for (int u = 0; u < NH; ++u) l = fmaf(h[u], __ldg(P + ag.o_pi_w + u * n_a + c), l);
+        for (int u = 0; u < H; ++u) l = fmaf(h[u], __ldg(P + ag.o_pi_w + u * n_a + c), l);
         l += __ldg(P + ag.o_pi_b + c);
         pi[c] = l;
         mx = fmaxf(mx, l);
@@ -298,8 +298,8 @@ __global__ void __launch_bounds__(16 * TY) cell_fwd_kernel(const __grid_constant
     float v = 0.f;
     if (MODE != MODE_P) {                                               // v = [h, onehot(a_j)] W_v + b  (policies.py:59-77)
 #pragma unroll
-      for (int u = 0; u < NH; ++u) v = fmaf(h[u], __ldg(P + ag.o_v_w + u), v);
-      for (int s = 0; s < ag.n_nbr; ++s) v += __ldg(P + ag.o_v_w + NH + s * n_a + a.act_in[(size_t)ag.nbr[s] * B + b]);
+      for (int u = 0; u < H; ++u) v = fmaf(h[u], __ldg(P + ag.o_v_w + u), v);
+      for (int s = 0; s < ag.n_nbr; ++s) v += __ldg(P + ag.o_v_w + H + s * n_a + a.act_in[(size_t)ag.nbr[s] * B + b]);
       v += __ldg(P + ag.o_v_b);
       if (a.v != nullptr) a.v[row] = v;
     }
@@ -346,13 +346,13 @@ __global__ void __launch_bounds__(16 * TY) cell_fwd_kernel(const __grid_constant
     float macc[TM][4];
 #pragma unroll
     for (int q = 0; q < TM; ++q) { macc[q][0] = macc[q][1] = macc[q][2] = macc[q][3] = 0.f; }
-    gemm_rowA<TM, 1, TY, KC>(macc, Hs, LDH, NH, P + ag.o_mfc_w, NH, WsE, tid);
+    gemm_rowA<TM, 1, TY, KC, H>(macc, Hs, LDH, H, P + ag.o_mfc_w, H, WsE, tid);
     const float4 bb = *reinterpret_cast<const float4*>(P + ag.o_mfc_b + 4 * tx);
 #pragma unroll
     for (int q = 0; q < TM; ++q) {
       const int r = ty + TY * q;
       if (r < rows)
-        *reinterpret_cast<float4*>(a.msg_out + ((size_t)i * B + b0 + r) * NH + 4 * tx) =
+        *reinterpret_cast<float4*>(a.msg_out + ((size_t)i * B + b0 + r) * H + 4 * tx) =
             make_float4(fmaxf(macc[q][0] + bb.x, 0.f), fmaxf(macc[q][1] + bb.y, 0.f), fmaxf(macc[q][2] + bb.z, 0.f),
                         fmaxf(macc[q][3] + bb.w, 0.f));
     }
@@ -360,33 +360,33 @@ __global__ void __launch_bounds__(16 * TY) cell_fwd_kernel(const __grid_constant
 }
 
 // stand-alone DIAL message kernel (after a reset / state load): msg = relu(h W_mfc + b)
-template <int BM, int TY>
-__global__ void __launch_bounds__(16 * TY) dial_msg_kernel(const __grid_constant__ nmarl_model m, int B,
+template <int BM, int TY, int H>
+__global__ void __launch_bounds__(H / 4 * TY) dial_msg_kernel(const __grid_constant__ nmarl_model m, int B,
                                                           const float* __restrict__ P, const float* __restrict__ h,
                                                           float* __restrict__ msg) {
-  constexpr int NT = 16 * TY, TM = BM / TY, KC = 16, LDH = NH + 4;
+  constexpr int NT = H / 4 * TY, TM = BM / TY, KC = 16, LDH = H + 4;
   __shared__ __align__(16) float Hs[BM * LDH];
-  __shared__ __align__(16) float Ws[2 * KC * NH];
+  __shared__ __align__(16) float Ws[2 * KC * H];
   const int i = blockIdx.y, b0 = blockIdx.x * BM, rows = min(BM, B - b0);
   const nmarl_agent& ag = m.agent[i];
-  const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
-  for (int idx = tid; idx < BM * (NH / 4); idx += NT) {
-    const int r = idx / (NH / 4), u4 = idx - r * (NH / 4);
+  const int tid = threadIdx.x, tx = tid & (H / 4 - 1), ty = tid >> nmarl_log2(H / 4);
+  for (int idx = tid; idx < BM * (H / 4); idx += NT) {
+    const int r = idx / (H / 4), u4 = idx - r * (H / 4);
     float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-    if (r < rows) v = *reinterpret_cast<const float4*>(h + ((size_t)i * B + b0 + r) * NH + 4 * u4);
+    if (r < rows) v = *reinterpret_cast<const float4*>(h + ((size_t)i * B + b0 + r) * H + 4 * u4);
     *reinterpret_cast<float4*>(Hs + r * LDH + 4 * u4) = v;
   }
   __syncthreads();
   float acc[TM][4];
 #pragma unroll
   for (int q = 0; q < TM; ++q) { acc[q][0] = acc[q][1] = acc[q][2] = acc[q][3] = 0.f; }
-  gemm_rowA<TM, 1, TY, KC>(acc, Hs, LDH, NH, P + ag.o_mfc_w, NH, Ws, tid);
+  gemm_rowA<TM, 1, TY, KC, H>(acc, Hs, LDH, H, P + ag.o_mfc_w, H, Ws, tid);
   const float4 bb = *reinterpret_cast<const float4*>(P + ag.o_mfc_b + 4 * tx);
 #pragma unroll
   for (int q = 0; q < TM; ++q) {
     const int r = ty + TY * q;
     if (r < rows)
-      *reinterpret_cast<float4*>(msg + ((size_t)i * B + b0 + r) * NH + 4 * tx) =
+      *reinterpret_cast<float4*>(msg + ((size_t)i * B + b0 + r) * H + 4 * tx) =
           make_float4(fmaxf(acc[q][0] + bb.x, 0.f), fmaxf(acc[q][1] + bb.y, 0.f), fmaxf(acc[q][2] + bb.z, 0.f),
                       fmaxf(acc[q][3] + bb.w, 0.f));
   }
@@ -396,14 +396,15 @@ __global__ void rng_advance_kernel(uint64_t* rng, uint64_t n) {
   if (threadIdx.x == 0 && blockIdx.x == 0) rng[1] += n;
 }
 
-constexpr int FWD_BM = 64, FWD_TY = 16;
+constexpr int FWD_BM = 64;
 NMARL_PARAMS_FIT(nmarl_model, FwdK);                                             // cell_fwd_kernel
 NMARL_PARAMS_FIT(nmarl_model, int, const float*, const float*, float*);          // dial_msg_kernel
 
-template <int VAR, int MODE>
+template <int VAR, int MODE, int H>
 int launch_fwd(const nmarl_model* m, const FwdK& k, cudaStream_t st) {
-  auto kern = cell_fwd_kernel<VAR, MODE, FWD_BM, FWD_TY>;
-  const size_t smem = fwd_smem_floats<FWD_BM, 16>(*m) * sizeof(float);
+  constexpr int TY = nmarl_ffma_ty(H);
+  auto kern = cell_fwd_kernel<VAR, MODE, FWD_BM, TY, H>;
+  const size_t smem = fwd_smem_floats<FWD_BM, 16, H>(*m) * sizeof(float);
   NMARL_CHECK(smem <= 227 * 1024, "policy_step: shared memory %zu B exceeds 227 KB", smem);
   static size_t configured = 0;     // per instantiation
   if (smem > configured) {
@@ -411,19 +412,30 @@ int launch_fwd(const nmarl_model* m, const FwdK& k, cudaStream_t st) {
     configured = smem;
   }
   dim3 grid((k.a.B + FWD_BM - 1) / FWD_BM, m->n_agent);
-  kern<<<grid, 16 * FWD_TY, smem, st>>>(*m, k);
+  kern<<<grid, H / 4 * TY, smem, st>>>(*m, k);
   NMARL_LAUNCH_CHECK();
   return 0;
+}
+
+template <int VAR, int MODE>
+int launch_fwd_width(const nmarl_model* m, const FwdK& k, cudaStream_t st) {
+  switch (nmarl_n_h(*m)) {
+    case 16: return launch_fwd<VAR, MODE, 16>(m, k, st);
+    case 32: return launch_fwd<VAR, MODE, 32>(m, k, st);
+    case 64: return launch_fwd<VAR, MODE, 64>(m, k, st);
+  }
+  nmarl_set_error("n_h %d has no FFMA kernel", nmarl_n_h(*m));
+  return 1;
 }
 
 template <int MODE>
 int dispatch_fwd(const nmarl_model* m, const FwdK& k, cudaStream_t st) {
   if (nmarl_tc_fwd_supported(m, &k.a)) return nmarl_tc_launch_fwd(m, k, MODE, st);
   switch (m->variant) {
-    case NMARL_IA2C: return launch_fwd<NMARL_IA2C, MODE>(m, k, st);
-    case NMARL_NC: return launch_fwd<NMARL_NC, MODE>(m, k, st);
-    case NMARL_IC3: return launch_fwd<NMARL_IC3, MODE>(m, k, st);
-    case NMARL_DIAL: return launch_fwd<NMARL_DIAL, MODE>(m, k, st);
+    case NMARL_IA2C: return launch_fwd_width<NMARL_IA2C, MODE>(m, k, st);
+    case NMARL_NC: return launch_fwd_width<NMARL_NC, MODE>(m, k, st);
+    case NMARL_IC3: return launch_fwd_width<NMARL_IC3, MODE>(m, k, st);
+    case NMARL_DIAL: return launch_fwd_width<NMARL_DIAL, MODE>(m, k, st);
   }
   nmarl_set_error("unknown variant %d", m->variant);
   return 1;
@@ -433,15 +445,17 @@ int check_model(const nmarl_model* m) {
   NMARL_CHECK(m != nullptr, "model is NULL");
   NMARL_CHECK(m->n_agent > 0 && m->n_agent <= NMARL_MAX_AGENT, "n_agent %d out of range", m->n_agent);
   NMARL_CHECK(m->n_a > 0 && m->n_a < NMARL_MAX_NA, "n_a %d out of range (max %d)", m->n_a, NMARL_MAX_NA - 1);
-  NMARL_CHECK(m->s_dim == ((m->variant == NMARL_NC) ? 3 * NH : NH), "s_dim %d does not match variant", m->s_dim);
+  const int H = nmarl_n_h(*m);
+  NMARL_CHECK(nmarl_width_ok(H) && m->s_dim == ((m->variant == NMARL_NC) ? 3 * H : H),
+              "s_dim %d: LSTM width n_h %d not supported (16, 32 or 64; s_dim = 3 * n_h for NeurComm, else n_h)", m->s_dim, H);
   NMARL_CHECK(m->kx_pad % 4 == 0 && m->kp_pad % 4 == 0 && m->km_pad % 4 == 0, "segment pads must be multiples of 4");
   for (int i = 0; i < m->n_agent; ++i) {
     const nmarl_agent& ag = m->agent[i];
     NMARL_CHECK(ag.n_nbr >= 0 && ag.n_nbr <= NMARL_MAX_NBR, "agent %d: n_nbr %d", i, ag.n_nbr);
     NMARL_CHECK(ag.x_nsrc * ag.x_w <= m->kx_pad, "agent %d: obs width exceeds kx_pad", i);
-    NMARL_CHECK((m->variant != NMARL_NC && m->variant != NMARL_DIAL) || ag.n_nbr * NH <= m->km_pad,
+    NMARL_CHECK((m->variant != NMARL_NC && m->variant != NMARL_DIAL) || ag.n_nbr * H <= m->km_pad,
                 "agent %d: message width exceeds km_pad", i);
-    NMARL_CHECK(m->variant != NMARL_IC3 || m->km_pad >= NH, "CommNet needs km_pad >= 64");
+    NMARL_CHECK(m->variant != NMARL_IC3 || m->km_pad >= H, "CommNet needs km_pad >= n_h (%d)", H);
     NMARL_CHECK(m->variant != NMARL_NC || ag.n_nbr * m->n_a <= m->kp_pad, "agent %d: fingerprint width exceeds kp_pad", i);
     NMARL_CHECK(m->variant != NMARL_IC3 || ag.n_nbr > 0, "agent %d: CommNet needs >= 1 neighbour", i);
     NMARL_CHECK(m->variant == NMARL_IA2C || ag.o_b_msg >= 0 || (m->variant == NMARL_DIAL && ag.n_nbr == 0),
@@ -508,7 +522,12 @@ extern "C" int nmarl_dial_msg(const nmarl_model* m, int B, const float* params, 
   if (check_model(m)) return 1;
   NMARL_CHECK(m->variant == NMARL_DIAL, "dial_msg: model is not DIAL");
   dim3 grid((B + 63) / 64, m->n_agent);
-  dial_msg_kernel<64, 16><<<grid, 256, 0, (cudaStream_t)stream>>>(*m, B, params, h, msg);
+  cudaStream_t st = (cudaStream_t)stream;
+  switch (nmarl_n_h(*m)) {
+    case 16: dial_msg_kernel<64, nmarl_ffma_ty(16), 16><<<grid, 256, 0, st>>>(*m, B, params, h, msg); break;
+    case 32: dial_msg_kernel<64, nmarl_ffma_ty(32), 32><<<grid, 256, 0, st>>>(*m, B, params, h, msg); break;
+    default: dial_msg_kernel<64, nmarl_ffma_ty(64), 64><<<grid, 256, 0, st>>>(*m, B, params, h, msg); break;
+  }
   NMARL_LAUNCH_CHECK();
   return 0;
 }

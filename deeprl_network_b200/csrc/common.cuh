@@ -5,8 +5,17 @@
 #include <stdio.h>
 #include "../../include/nmarl.h"
 
-#define NH NMARL_NH          // 64
+#define NH NMARL_NH          // 64: the width the tensor-core kernels are built for
 #define NG (4 * NMARL_NH)    // 256 gate columns, order i,f,o,u (agents/utils.py:106,202)
+
+// LSTM widths the FP32-FFMA kernels are instantiated for (nmarl_n_h); the kernels below take the width as a
+// template parameter H and the host dispatches on nmarl_n_h(*m).  Thread blocks keep 256 threads at every width: H/4 threads
+// span a row's columns (4 each) and 1024/H thread rows cover the tile.
+__host__ __device__ constexpr bool nmarl_width_ok(int h) { return h == 16 || h == 32 || h == 64; }
+// n_h from the descriptor: s_dim = 3 * n_h for NeurComm ([s_x | s_p | s_m]), n_h for every other cell
+__host__ __device__ inline int nmarl_n_h(const nmarl_model& m) { return m.variant == NMARL_NC ? m.s_dim / 3 : m.s_dim; }
+constexpr int nmarl_ffma_ty(int h) { return 1024 / h; }
+__host__ __device__ constexpr int nmarl_log2(int x) { return x <= 1 ? 0 : 1 + nmarl_log2(x / 2); }
 
 void nmarl_set_error(const char* fmt, ...);
 
@@ -95,22 +104,23 @@ __device__ __forceinline__ float f4get(const float4& v, int k) {
   return k == 0 ? v.x : (k == 1 ? v.y : (k == 2 ? v.z : v.w));
 }
 
-// ---- FP32 FFMA tile GEMM: acc[TM][4*NGRP] += A_tile[BM x K] * W[K x 64*NGRP] ----------------
-// Thread layout: 16 (tx) x TY (ty) threads; thread rows = ty + TY*q (q<TM), thread columns =
-// g*64 + 4*tx + j (g<NGRP, j<4) -- for the LSTM gate GEMM (NGRP=4) a thread therefore owns all
-// four gates i,f,o,u of 4 hidden units and the cell update is a pure register epilogue.
+// ---- FP32 FFMA tile GEMM: acc[TM][4*NGRP] += A_tile[BM x K] * W[K x W*NGRP] ----------------
+// Thread layout: W/4 (tx) x TY (ty) threads; thread rows = ty + TY*q (q<TM), thread columns =
+// g*W + 4*tx + j (g<NGRP, j<4) -- W is the LSTM width n_h, so for the gate GEMM (NGRP=4) a thread
+// owns all four gates i,f,o,u of 4 hidden units and the cell update is a pure register epilogue.
 // A: shared memory, row-major [BM][lda] (lda % 4 == 0, columns [K, roundup4(K)) zeroed).
 // W: global memory, k-major [K][ldw] (ldw % 4 == 0, 16B-aligned), streamed through a 2-stage
-//    cp.async ring Ws[2][KC][64*NGRP]; rows >= K are zero-filled.
+//    cp.async ring Ws[2][KC][W*NGRP]; rows >= K are zero-filled.
 // Accumulation is k-ascending FFMA (fixed order -> run-to-run deterministic).
 // Every thread of the CTA must call this (it contains __syncthreads()).
-template <int TM, int NGRP, int TY, int KC>
+template <int TM, int NGRP, int TY, int KC, int CW>
 __device__ __forceinline__ void gemm_rowA(float (&acc)[TM][4 * NGRP], const float* As, int lda, int K,
                                           const float* __restrict__ W, int ldw, float* Ws, int tid) {
-  constexpr int NT = 16 * TY;
-  constexpr int WROW = 64 * NGRP;
-  constexpr int F4ROW = 16 * NGRP;
-  const int tx = tid & 15, ty = tid >> 4;
+  constexpr int TXN = CW / 4;
+  constexpr int NT = TXN * TY;
+  constexpr int WROW = CW * NGRP;
+  constexpr int F4ROW = TXN * NGRP;
+  const int tx = tid & (TXN - 1), ty = tid >> nmarl_log2(TXN);
   const int Kpad = (K + 3) & ~3;
   const int nch = (Kpad + KC - 1) / KC;
   auto load = [&](int ch, int st) {
@@ -144,7 +154,7 @@ __device__ __forceinline__ void gemm_rowA(float (&acc)[TM][4 * NGRP], const floa
         float4 b[NGRP];
 #pragma unroll
         for (int g = 0; g < NGRP; ++g)
-          b[g] = *reinterpret_cast<const float4*>(Wst + (k4 + kk) * WROW + g * 64 + 4 * tx);
+          b[g] = *reinterpret_cast<const float4*>(Wst + (k4 + kk) * WROW + g * CW + 4 * tx);
 #pragma unroll
         for (int q = 0; q < TM; ++q) {
           const float av = f4get(a[q], kk);

@@ -511,7 +511,7 @@ int launch_tc_mode(const nmarl_model* m, const FwdK& k, int mode, cudaStream_t s
 }  // namespace
 
 bool nmarl_tc_fwd_supported(const nmarl_model* m, const nmarl_fwd_args* a) {
-  if (a->wpack == nullptr || a->B % 128 != 0 || m->kx_pad > 32 || m->kp_pad > 32) return false;
+  if (a->wpack == nullptr || a->B % 128 != 0 || m->kx_pad > 32 || m->kp_pad > 32 || nmarl_n_h(*m) != NMARL_NH) return false;
   for (int i = 0; i < m->n_agent; ++i)
     if (m->agent[i].tp_g < 0 || m->agent[i].tp_x < 0) return false;
   return true;
@@ -582,6 +582,7 @@ NMARL_PARAMS_FIT(nmarl_model, const float*, float*);                            
 
 extern "C" int nmarl_pack_weights(const nmarl_model* m, const float* params, float* wt, float* wpack, void* stream) {
   NMARL_CHECK(m && params && wt && wpack, "pack_weights: missing buffers");
+  NMARL_CHECK(nmarl_n_h(*m) == NMARL_NH, "pack_weights: the tensor-core kernels need n_h = %d (got %d)", NMARL_NH, nmarl_n_h(*m));
   cudaStream_t st = (cudaStream_t)stream;
   pack_all_kernel<<<dim3(16, m->n_agent * PACK_JOBS), 256, 0, st>>>(*m, params, wpack);
   NMARL_LAUNCH_CHECK();

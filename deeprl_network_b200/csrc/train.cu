@@ -77,10 +77,11 @@ __global__ void __launch_bounds__(256) transpose_all_kernel(const __grid_constan
   const int j = blockIdx.z, i = blockIdx.y;
   if (!(jobs & (1 << j))) return;
   const nmarl_agent& ag = m.agent[i];
-  int rows = 0, cols = NH, src_off = 0, dst_off = 0;
-  if (j == 0) { rows = m.s_dim + NH; cols = NG; src_off = ag.o_wxh; dst_off = ag.t_wxh; }
-  else if (j == 1) { rows = (m.variant == NMARL_IC3) ? NH : ag.n_nbr * NH; src_off = ag.o_w_msg; dst_off = ag.t_w_msg; }
-  else { rows = NH; src_off = ag.o_mfc_w; dst_off = ag.t_mfc; }
+  const int H = nmarl_n_h(m);
+  int rows = 0, cols = H, src_off = 0, dst_off = 0;
+  if (j == 0) { rows = m.s_dim + H; cols = 4 * H; src_off = ag.o_wxh; dst_off = ag.t_wxh; }
+  else if (j == 1) { rows = (m.variant == NMARL_IC3) ? H : ag.n_nbr * H; src_off = ag.o_w_msg; dst_off = ag.t_w_msg; }
+  else { rows = H; src_off = ag.o_mfc_w; dst_off = ag.t_mfc; }
   const float* __restrict__ src = params + src_off;
   float* __restrict__ dst = wt + dst_off;
   const int tx = (cols + 31) / 32, ntile = tx * ((rows + 31) / 32);
@@ -100,20 +101,20 @@ __global__ void __launch_bounds__(256) transpose_all_kernel(const __grid_constan
 }
 
 // ============================ K9: one reverse step of the cell ==================================
-template <int VAR, int BM, int TY>
-__global__ void __launch_bounds__(16 * TY) cell_bwd_kernel(const __grid_constant__ nmarl_model m,
+template <int VAR, int BM, int TY, int H>
+__global__ void __launch_bounds__(H / 4 * TY) cell_bwd_kernel(const __grid_constant__ nmarl_model m,
                                                           const __grid_constant__ BwdK k) {
-  constexpr int NT = 16 * TY, TM = BM / TY, KC = 16;
+  constexpr int TM = BM / TY, KC = 16;
   constexpr int NGRP = (VAR == NMARL_NC) ? 4 : 2;
-  constexpr int LDZ = NG + 4, LDP = NH + 4;
+  constexpr int LDZ = (4 * H) + 4, LDP = H + 4;
   extern __shared__ __align__(16) float smem[];
   float* DZ = smem;                         // [BM][LDZ]
-  float* Ws = smem + (size_t)BM * LDZ;      // 2*KC*64*NGRP
+  float* Ws = smem + (size_t)BM * LDZ;      // 2*KC*H*NGRP
   float* DPm = smem;                        // aliases DZ after the dgrad GEMM
   const int i = blockIdx.y;
   const nmarl_agent& ag = m.agent[i];
   const int B = k.B, b0 = blockIdx.x * BM, rows = min(BM, B - b0);
-  const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
+  const int tid = threadIdx.x, tx = tid & (H / 4 - 1), ty = tid >> nmarl_log2(H / 4);
   const int n_a = m.n_a, SD = m.s_dim;
   const float* __restrict__ P = k.params;
 
@@ -148,24 +149,24 @@ __global__ void __launch_bounds__(16 * TY) cell_bwd_kernel(const __grid_constant
         dh[j] = fmaf(dv, wpi[j][NMARL_MAX_NA - 1], s);
       }
       if (k.has_next) {
-        const float4 r4 = *reinterpret_cast<const float4*>(k.dh_in + row * NH + 4 * tx);
+        const float4 r4 = *reinterpret_cast<const float4*>(k.dh_in + row * H + 4 * tx);
         dh[0] += r4.x; dh[1] += r4.y; dh[2] += r4.z; dh[3] += r4.w;
         if (VAR == NMARL_NC || VAR == NMARL_IC3) {
           for (int s = 0; s < ag.n_recv; ++s) {
             const float4 m4 = *reinterpret_cast<const float4*>(
-                k.dmsg_in + (((size_t)ag.recv_agent[s] * NMARL_MAX_NBR + ag.recv_slot[s]) * B + b) * NH + 4 * tx);
+                k.dmsg_in + (((size_t)ag.recv_agent[s] * NMARL_MAX_NBR + ag.recv_slot[s]) * B + b) * H + 4 * tx);
             dh[0] += m4.x; dh[1] += m4.y; dh[2] += m4.z; dh[3] += m4.w;
           }
         }
-        const float4 c4 = *reinterpret_cast<const float4*>(k.dc_in + row * NH + 4 * tx);
+        const float4 c4 = *reinterpret_cast<const float4*>(k.dc_in + row * H + 4 * tx);
         dc[0] = c4.x; dc[1] = c4.y; dc[2] = c4.z; dc[3] = c4.w;
       }
       const float nd = 1.0f - k.done_pre[b];
-      const float* gs = k.sv_gates + row * NG + 4 * tx;
-      const float4 gi = *reinterpret_cast<const float4*>(gs), gf = *reinterpret_cast<const float4*>(gs + NH),
-                   go = *reinterpret_cast<const float4*>(gs + 2 * NH), gu = *reinterpret_cast<const float4*>(gs + 3 * NH);
-      const float4 cc = *reinterpret_cast<const float4*>(k.c_cur + row * NH + 4 * tx);
-      const float4 cp = *reinterpret_cast<const float4*>(k.c_prev + row * NH + 4 * tx);
+      const float* gs = k.sv_gates + row * (4 * H) + 4 * tx;
+      const float4 gi = *reinterpret_cast<const float4*>(gs), gf = *reinterpret_cast<const float4*>(gs + H),
+                   go = *reinterpret_cast<const float4*>(gs + 2 * H), gu = *reinterpret_cast<const float4*>(gs + 3 * H);
+      const float4 cc = *reinterpret_cast<const float4*>(k.c_cur + row * H + 4 * tx);
+      const float4 cp = *reinterpret_cast<const float4*>(k.c_prev + row * H + 4 * tx);
       float dcp[4];
 #pragma unroll
       for (int j = 0; j < 4; ++j) {
@@ -179,15 +180,15 @@ __global__ void __launch_bounds__(16 * TY) cell_bwd_kernel(const __grid_constant
         dz[3][j] = dct * ig * (1.0f - ug * ug);
         dcp[j] = dct * fg * nd;
       }
-      *reinterpret_cast<float4*>(k.dc_out + row * NH + 4 * tx) = make_float4(dcp[0], dcp[1], dcp[2], dcp[3]);
-      float* zo = k.sv_dz + row * NG + 4 * tx;
+      *reinterpret_cast<float4*>(k.dc_out + row * H + 4 * tx) = make_float4(dcp[0], dcp[1], dcp[2], dcp[3]);
+      float* zo = k.sv_dz + row * (4 * H) + 4 * tx;
 #pragma unroll
       for (int g = 0; g < 4; ++g)
-        *reinterpret_cast<float4*>(zo + g * NH) = make_float4(dz[g][0], dz[g][1], dz[g][2], dz[g][3]);
+        *reinterpret_cast<float4*>(zo + g * H) = make_float4(dz[g][0], dz[g][1], dz[g][2], dz[g][3]);
     }
 #pragma unroll
     for (int g = 0; g < 4; ++g)
-      *reinterpret_cast<float4*>(DZ + r * LDZ + g * NH + 4 * tx) = make_float4(dz[g][0], dz[g][1], dz[g][2], dz[g][3]);
+      *reinterpret_cast<float4*>(DZ + r * LDZ + g * H + 4 * tx) = make_float4(dz[g][0], dz[g][1], dz[g][2], dz[g][3]);
   }
   __syncthreads();
 
@@ -197,7 +198,7 @@ __global__ void __launch_bounds__(16 * TY) cell_bwd_kernel(const __grid_constant
   for (int q = 0; q < TM; ++q)
 #pragma unroll
     for (int c = 0; c < 4 * NGRP; ++c) acc[q][c] = 0.f;
-  gemm_rowA<TM, NGRP, TY, KC>(acc, DZ, LDZ, NG, k.wt + ag.t_wxh, SD + NH, Ws, tid);
+  gemm_rowA<TM, NGRP, TY, KC, H>(acc, DZ, LDZ, (4 * H), k.wt + ag.t_wxh, SD + H, Ws, tid);
 #pragma unroll
   for (int q = 0; q < TM; ++q) {
     const int r = ty + TY * q;
@@ -207,36 +208,36 @@ __global__ void __launch_bounds__(16 * TY) cell_bwd_kernel(const __grid_constant
       const size_t row = (size_t)i * B + b;
       const float nd = 1.0f - k.done_pre[b];
       constexpr int GH = 4 * (NGRP - 1);
-      *reinterpret_cast<float4*>(k.dh_out + row * NH + 4 * tx) =
+      *reinterpret_cast<float4*>(k.dh_out + row * H + 4 * tx) =
           make_float4(acc[q][GH] * nd, acc[q][GH + 1] * nd, acc[q][GH + 2] * nd, acc[q][GH + 3] * nd);
-      float* dp = k.sv_dpre + row * 192 + 4 * tx;
+      float* dp = k.sv_dpre + row * (3 * H) + 4 * tx;
       if (VAR == NMARL_NC) {
-        const float* sp = k.sv_sh + row * (SD + NH) + 4 * tx;
+        const float* sp = k.sv_sh + row * (SD + H) + 4 * tx;
 #pragma unroll
         for (int g = 0; g < 3; ++g) {
-          const float4 s4 = *reinterpret_cast<const float4*>(sp + g * NH);
+          const float4 s4 = *reinterpret_cast<const float4*>(sp + g * H);
           float o[4];
 #pragma unroll
           for (int j = 0; j < 4; ++j) o[j] = f4get(s4, j) > 0.f ? acc[q][4 * g + j] : 0.f;
-          *reinterpret_cast<float4*>(dp + g * NH) = make_float4(o[0], o[1], o[2], o[3]);
+          *reinterpret_cast<float4*>(dp + g * H) = make_float4(o[0], o[1], o[2], o[3]);
           if (g == 2) { dpm[0] = o[0]; dpm[1] = o[1]; dpm[2] = o[2]; dpm[3] = o[3]; }
         }
       } else if (VAR == NMARL_IA2C) {
-        const float4 s4 = *reinterpret_cast<const float4*>(k.sv_sh + row * (SD + NH) + 4 * tx);
+        const float4 s4 = *reinterpret_cast<const float4*>(k.sv_sh + row * (SD + H) + 4 * tx);
         float o[4];
 #pragma unroll
         for (int j = 0; j < 4; ++j) o[j] = f4get(s4, j) > 0.f ? acc[q][j] : 0.f;
         *reinterpret_cast<float4*>(dp) = make_float4(o[0], o[1], o[2], o[3]);
       } else if (VAR == NMARL_IC3) {
-        const float4 hx = *reinterpret_cast<const float4*>(k.sv_enc + row * 128 + 4 * tx);
+        const float4 hx = *reinterpret_cast<const float4*>(k.sv_enc + row * (2 * H) + 4 * tx);
         float o[4];
 #pragma unroll
         for (int j = 0; j < 4; ++j) { const float x = f4get(hx, j); o[j] = acc[q][j] * (1.0f - x * x); dpm[j] = acc[q][j]; }
         *reinterpret_cast<float4*>(dp) = make_float4(o[0], o[1], o[2], o[3]);
-        *reinterpret_cast<float4*>(dp + NH) = make_float4(dpm[0], dpm[1], dpm[2], dpm[3]);
+        *reinterpret_cast<float4*>(dp + H) = make_float4(dpm[0], dpm[1], dpm[2], dpm[3]);
       } else {  // DIAL
-        const float4 hx = *reinterpret_cast<const float4*>(k.sv_enc + row * 128 + 4 * tx);
-        const float4 hm = *reinterpret_cast<const float4*>(k.sv_enc + row * 128 + NH + 4 * tx);
+        const float4 hx = *reinterpret_cast<const float4*>(k.sv_enc + row * (2 * H) + 4 * tx);
+        const float4 hm = *reinterpret_cast<const float4*>(k.sv_enc + row * (2 * H) + H + 4 * tx);
         float o[4];
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
@@ -244,7 +245,7 @@ __global__ void __launch_bounds__(16 * TY) cell_bwd_kernel(const __grid_constant
           dpm[j] = f4get(hm, j) > 0.f ? acc[q][j] : 0.f;
         }
         *reinterpret_cast<float4*>(dp) = make_float4(o[0], o[1], o[2], o[3]);
-        *reinterpret_cast<float4*>(dp + NH) = make_float4(dpm[0], dpm[1], dpm[2], dpm[3]);
+        *reinterpret_cast<float4*>(dp + H) = make_float4(dpm[0], dpm[1], dpm[2], dpm[3]);
       }
     }
     if (VAR != NMARL_IA2C) *reinterpret_cast<float4*>(DPm + r * LDP + 4 * tx) = make_float4(dpm[0], dpm[1], dpm[2], dpm[3]);
@@ -252,13 +253,13 @@ __global__ void __launch_bounds__(16 * TY) cell_bwd_kernel(const __grid_constant
 
   // ---- phase 3: message gradient  dm = dpre_m W_msg^T, one 64-wide block per neighbour slot ------
   if (VAR != NMARL_IA2C) {
-    const int Km = (VAR == NMARL_IC3) ? NH : ag.n_nbr * NH;
+    const int Km = (VAR == NMARL_IC3) ? H : ag.n_nbr * H;
     const int nblk = (VAR == NMARL_IC3) ? 1 : ag.n_nbr;
     for (int s = 0; s < nblk; ++s) {
       float a2[TM][4];
 #pragma unroll
       for (int q = 0; q < TM; ++q) { a2[q][0] = a2[q][1] = a2[q][2] = a2[q][3] = 0.f; }
-      gemm_rowA<TM, 1, TY, KC>(a2, DPm, LDP, NH, k.wt + ag.t_w_msg + s * NH, Km, Ws, tid);
+      gemm_rowA<TM, 1, TY, KC, H>(a2, DPm, LDP, H, k.wt + ag.t_w_msg + s * H, Km, Ws, tid);
 #pragma unroll
       for (int q = 0; q < TM; ++q) {
         const int r = ty + TY * q;
@@ -268,9 +269,9 @@ __global__ void __launch_bounds__(16 * TY) cell_bwd_kernel(const __grid_constant
           const float nn = (float)ag.n_nbr;
           const float4 o = make_float4(a2[q][0] / nn, a2[q][1] / nn, a2[q][2] / nn, a2[q][3] / nn);
           for (int s2 = 0; s2 < ag.n_nbr; ++s2)
-            *reinterpret_cast<float4*>(k.dmsg_out + (((size_t)i * NMARL_MAX_NBR + s2) * B + b) * NH + 4 * tx) = o;
+            *reinterpret_cast<float4*>(k.dmsg_out + (((size_t)i * NMARL_MAX_NBR + s2) * B + b) * H + 4 * tx) = o;
         } else {
-          *reinterpret_cast<float4*>(k.dmsg_out + (((size_t)i * NMARL_MAX_NBR + s) * B + b) * NH + 4 * tx) =
+          *reinterpret_cast<float4*>(k.dmsg_out + (((size_t)i * NMARL_MAX_NBR + s) * B + b) * H + 4 * tx) =
               make_float4(a2[q][0], a2[q][1], a2[q][2], a2[q][3]);
         }
       }
@@ -280,31 +281,31 @@ __global__ void __launch_bounds__(16 * TY) cell_bwd_kernel(const __grid_constant
 
 // DIAL: sender-side message fc backward at step t (after cell_bwd(t)):
 //   dmp = (sum over receivers of dmsg) * relu'(msg_t);  dh_rec += dmp W_mfc^T
-template <int BM, int TY>
-__global__ void __launch_bounds__(16 * TY) dial_msg_bwd_kernel(const __grid_constant__ nmarl_model m, int B,
+template <int BM, int TY, int H>
+__global__ void __launch_bounds__(H / 4 * TY) dial_msg_bwd_kernel(const __grid_constant__ nmarl_model m, int B,
                                                               const float* __restrict__ wt,
                                                               const float* __restrict__ msg_t,
                                                               const float* __restrict__ dmsg, float* __restrict__ sv_dmp,
                                                               float* __restrict__ dh_rec) {
-  constexpr int NT = 16 * TY, TM = BM / TY, KC = 16, LDP = NH + 4;
+  constexpr int NT = H / 4 * TY, TM = BM / TY, KC = 16, LDP = H + 4;
   __shared__ __align__(16) float DM[BM * LDP];
-  __shared__ __align__(16) float Ws[2 * KC * NH];
+  __shared__ __align__(16) float Ws[2 * KC * H];
   const int i = blockIdx.y, b0 = blockIdx.x * BM, rows = min(BM, B - b0);
   const nmarl_agent& ag = m.agent[i];
-  const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
-  for (int idx = tid; idx < BM * (NH / 4); idx += NT) {
-    const int r = idx / (NH / 4), u4 = idx - r * (NH / 4);
+  const int tid = threadIdx.x, tx = tid & (H / 4 - 1), ty = tid >> nmarl_log2(H / 4);
+  for (int idx = tid; idx < BM * (H / 4); idx += NT) {
+    const int r = idx / (H / 4), u4 = idx - r * (H / 4);
     float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
     if (r < rows) {
       const int b = b0 + r;
       for (int s = 0; s < ag.n_recv; ++s) {
         const float4 w = *reinterpret_cast<const float4*>(
-            dmsg + (((size_t)ag.recv_agent[s] * NMARL_MAX_NBR + ag.recv_slot[s]) * B + b) * NH + 4 * u4);
+            dmsg + (((size_t)ag.recv_agent[s] * NMARL_MAX_NBR + ag.recv_slot[s]) * B + b) * H + 4 * u4);
         v.x += w.x; v.y += w.y; v.z += w.z; v.w += w.w;
       }
-      const float4 mm = *reinterpret_cast<const float4*>(msg_t + ((size_t)i * B + b) * NH + 4 * u4);
+      const float4 mm = *reinterpret_cast<const float4*>(msg_t + ((size_t)i * B + b) * H + 4 * u4);
       v.x = mm.x > 0.f ? v.x : 0.f; v.y = mm.y > 0.f ? v.y : 0.f; v.z = mm.z > 0.f ? v.z : 0.f; v.w = mm.w > 0.f ? v.w : 0.f;
-      *reinterpret_cast<float4*>(sv_dmp + ((size_t)i * B + b) * NH + 4 * u4) = v;
+      *reinterpret_cast<float4*>(sv_dmp + ((size_t)i * B + b) * H + 4 * u4) = v;
     }
     *reinterpret_cast<float4*>(DM + r * LDP + 4 * u4) = v;
   }
@@ -312,12 +313,12 @@ __global__ void __launch_bounds__(16 * TY) dial_msg_bwd_kernel(const __grid_cons
   float acc[TM][4];
 #pragma unroll
   for (int q = 0; q < TM; ++q) { acc[q][0] = acc[q][1] = acc[q][2] = acc[q][3] = 0.f; }
-  gemm_rowA<TM, 1, TY, KC>(acc, DM, LDP, NH, wt + ag.t_mfc, NH, Ws, tid);
+  gemm_rowA<TM, 1, TY, KC, H>(acc, DM, LDP, H, wt + ag.t_mfc, H, Ws, tid);
 #pragma unroll
   for (int q = 0; q < TM; ++q) {
     const int r = ty + TY * q;
     if (r < rows) {
-      float4* p = reinterpret_cast<float4*>(dh_rec + ((size_t)i * B + b0 + r) * NH + 4 * tx);
+      float4* p = reinterpret_cast<float4*>(dh_rec + ((size_t)i * B + b0 + r) * H + 4 * tx);
       float4 o = *p;
       o.x += acc[q][0]; o.y += acc[q][1]; o.z += acc[q][2]; o.w += acc[q][3];
       *p = o;
@@ -329,15 +330,22 @@ __global__ void __launch_bounds__(16 * TY) dial_msg_bwd_kernel(const __grid_cons
 struct WgK {
   int N, B, T, splits;
   const float* A; int lda; int a_col0;       // A[t][agent][env][lda], columns a_col0 + [0, Ka_i)
-  const float* D; int ldd; int d_col0;       // D[t][agent][env][ldd], columns d_col0 + [0, 64*NGRP)
+  const float* D; int ldd; int d_col0;       // D[t][agent][env][ldd], columns d_col0 + [0, ND)
   int ka_max;                                // workspace row count per (split, agent) = ka_max + 1 (bias row)
   int Ka[NMARL_MAX_AGENT];
-  float* ws;                                 // [splits][N][ka_max + 1][64*NGRP]
+  float* ws;                                 // [splits][N][ka_max + 1][ND]
 };
 
-template <int NGRP>
+// ND output columns (4 * n_h gate columns or n_h encoder columns).  A thread owns a 4 x 4 block per column group of
+// CW = min(ND, 64) columns, so 16 * CW / 4 threads cover the 64-row A tile.  Narrow outputs (ND = 16 / 32) leave the
+// rest of the 256 threads as RG further row groups: group p takes rows rr = p, p + RG, ... of every chunk, and the
+// groups' sums are added in group order at the end (fixed order -> deterministic).  ND >= 64 has one group.
+template <int ND>
 __global__ void __launch_bounds__(256) wgrad_kernel(const __grid_constant__ WgK k) {
-  constexpr int RC = 32, ND = 64 * NGRP;
+  constexpr int RC = 32;
+  constexpr int CW = ND < 64 ? ND : 64, NGRP = ND / CW, TXN = CW / 4;
+  constexpr int GT = 16 * TXN, RG = 256 / GT;
+  static_assert(RG >= 1 && RG <= 4 && NGRP * CW == ND, "wgrad: unsupported column count");
   extern __shared__ __align__(16) float wg_smem[];
   float (*As)[RC][64] = reinterpret_cast<float (*)[RC][64]>(wg_smem);
   float (*Ds)[RC][ND] = reinterpret_cast<float (*)[RC][ND]>(wg_smem + 2 * RC * 64);
@@ -346,7 +354,9 @@ __global__ void __launch_bounds__(256) wgrad_kernel(const __grid_constant__ WgK 
   // mt == 0 always runs: it writes the bias row, which wgrad_reduce_kernel reads even when Ka == 0 (an agent without
   // neighbours has no fingerprint / message inputs, but its encoder biases still get the column sums of D)
   if (mt > 0 && mt * 64 >= Ka) return;
-  const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
+  const int tid = threadIdx.x;
+  const int grp = (RG == 1) ? 0 : tid >> nmarl_log2(GT), gt = (RG == 1) ? tid : tid & (GT - 1);
+  const int tx = gt & (TXN - 1), ty = gt >> nmarl_log2(TXN);
   const int R = k.T * k.B;
   const int per = ((R + k.splits - 1) / k.splits + RC - 1) / RC * RC;
   const int r_begin = sp * per, r_end = min(R, r_begin + per);
@@ -370,8 +380,8 @@ __global__ void __launch_bounds__(256) wgrad_kernel(const __grid_constant__ WgK 
       const float* src = k.A + (((size_t)t * k.N + i) * k.B + b) * k.lda + k.a_col0 + col;
       cp_async16(&As[st][rr][4 * c4], ok ? src : k.A, ok ? 16 : 0);
     }
-    for (int idx = tid; idx < RC * 16 * NGRP; idx += 256) {   // D chunk: RC x ND
-      const int rr = idx / (16 * NGRP), c4 = idx - rr * (16 * NGRP);
+    for (int idx = tid; idx < RC * (ND / 4); idx += 256) {    // D chunk: RC x ND
+      const int rr = idx / (ND / 4), c4 = idx - rr * (ND / 4);
       const int r = rb + rr;
       const bool ok = r < r_end;
       const int t = ok ? r / k.B : 0, b = ok ? r - t * k.B : 0;
@@ -386,11 +396,11 @@ __global__ void __launch_bounds__(256) wgrad_kernel(const __grid_constant__ WgK 
     __syncthreads();
     const int st = ch & 1;
 #pragma unroll 8
-    for (int rr = 0; rr < RC; ++rr) {
+    for (int rr = grp; rr < RC; rr += RG) {
       const float4 a = *reinterpret_cast<const float4*>(&As[st][rr][4 * ty]);
       float4 d[NGRP];
 #pragma unroll
-      for (int g = 0; g < NGRP; ++g) d[g] = *reinterpret_cast<const float4*>(&Ds[st][rr][g * 64 + 4 * tx]);
+      for (int g = 0; g < NGRP; ++g) d[g] = *reinterpret_cast<const float4*>(&Ds[st][rr][g * CW + 4 * tx]);
 #pragma unroll
       for (int g = 0; g < NGRP; ++g) {
 #pragma unroll
@@ -403,39 +413,65 @@ __global__ void __launch_bounds__(256) wgrad_kernel(const __grid_constant__ WgK 
         }
       }
     }
-    if (mt == 0) {                                            // bias = column sums of D (rows rr = ty, ty+16)
+    if (mt == 0) {                                            // bias = column sums of D (rows y, y + 16*RG, ...)
+      const int y = grp * 16 + ty;
 #pragma unroll
-      for (int h2 = 0; h2 < RC / 16; ++h2) {
+      for (int h2 = 0; h2 < (RC + 16 * RG - 1) / (16 * RG); ++h2) {
+        const int rr = y + 16 * RG * h2;
+        if (rr < RC) {
 #pragma unroll
-        for (int g = 0; g < NGRP; ++g) {
-          const float4 d = *reinterpret_cast<const float4*>(&Ds[st][ty + 16 * h2][g * 64 + 4 * tx]);
-          bsum[4 * g] += d.x; bsum[4 * g + 1] += d.y; bsum[4 * g + 2] += d.z; bsum[4 * g + 3] += d.w;
+          for (int g = 0; g < NGRP; ++g) {
+            const float4 d = *reinterpret_cast<const float4*>(&Ds[st][rr][g * CW + 4 * tx]);
+            bsum[4 * g] += d.x; bsum[4 * g + 1] += d.y; bsum[4 * g + 2] += d.z; bsum[4 * g + 3] += d.w;
+          }
         }
       }
     }
     __syncthreads();
   }
-  float* wsb = k.ws + ((size_t)sp * k.N + i) * (size_t)(k.ka_max + 1) * ND;
+  if (RG > 1) {                                               // row groups 1.. -> group 0, in group order
+    float* part = &As[0][0][0];                               // (RG-1)*64*ND <= 2*RC*64 floats
+    if (grp > 0) {
 #pragma unroll
-  for (int mi = 0; mi < 4; ++mi) {
-    const int row = mt * 64 + 4 * ty + mi;
-    if (row < Ka) {
+      for (int mi = 0; mi < 4; ++mi)
+        *reinterpret_cast<float4*>(part + ((size_t)(grp - 1) * 64 + 4 * ty + mi) * ND + 4 * tx) =
+            make_float4(acc[mi][0], acc[mi][1], acc[mi][2], acc[mi][3]);
+    }
+    __syncthreads();
+    if (grp == 0) {
+      for (int p = 1; p < RG; ++p) {
 #pragma unroll
-      for (int g = 0; g < NGRP; ++g)
-        *reinterpret_cast<float4*>(wsb + (size_t)row * ND + g * 64 + 4 * tx) =
-            make_float4(acc[mi][4 * g], acc[mi][4 * g + 1], acc[mi][4 * g + 2], acc[mi][4 * g + 3]);
+        for (int mi = 0; mi < 4; ++mi) {
+          const float4 o = *reinterpret_cast<const float4*>(part + ((size_t)(p - 1) * 64 + 4 * ty + mi) * ND + 4 * tx);
+          acc[mi][0] += o.x; acc[mi][1] += o.y; acc[mi][2] += o.z; acc[mi][3] += o.w;
+        }
+      }
     }
   }
-  if (mt == 0) {                                              // reduce bias partials over ty (fixed order)
-    float* red = &Ds[0][0][0];                                // 2*RC*ND >= 16*ND floats
+  float* wsb = k.ws + ((size_t)sp * k.N + i) * (size_t)(k.ka_max + 1) * ND;
+  if (grp == 0) {
+#pragma unroll
+    for (int mi = 0; mi < 4; ++mi) {
+      const int row = mt * 64 + 4 * ty + mi;
+      if (row < Ka) {
+#pragma unroll
+        for (int g = 0; g < NGRP; ++g)
+          *reinterpret_cast<float4*>(wsb + (size_t)row * ND + g * CW + 4 * tx) =
+              make_float4(acc[mi][4 * g], acc[mi][4 * g + 1], acc[mi][4 * g + 2], acc[mi][4 * g + 3]);
+      }
+    }
+  }
+  if (mt == 0) {                                              // reduce bias partials over y (fixed order)
+    float* red = &Ds[0][0][0];                                // 2*RC*ND >= 16*RG*ND floats
+    const int y = grp * 16 + ty;
 #pragma unroll
     for (int g = 0; g < NGRP; ++g)
-      *reinterpret_cast<float4*>(red + ty * ND + g * 64 + 4 * tx) =
+      *reinterpret_cast<float4*>(red + y * ND + g * CW + 4 * tx) =
           make_float4(bsum[4 * g], bsum[4 * g + 1], bsum[4 * g + 2], bsum[4 * g + 3]);
     __syncthreads();
     for (int c = tid; c < ND; c += 256) {
       float s = 0.f;
-      for (int y = 0; y < 16; ++y) s += red[y * ND + c];
+      for (int y2 = 0; y2 < 16 * RG; ++y2) s += red[y2 * ND + c];
       wsb[(size_t)k.ka_max * ND + c] = s;
     }
   }
@@ -468,67 +504,72 @@ __global__ void wgrad_reduce_kernel(const __grid_constant__ WgRedK k) {
 // heads: dW_pi = h^T dlogits, db_pi, dW_v = [h, onehot(a_nbr)]^T dv, db_v   (skinny; own kernel)
 struct HeadK {
   int N, B, T, splits, n_a, fm;
-  const float* h1;           // h_seq + N*B*64  (h_t, t = 0..T-1)
+  const float* h1;           // h_seq + N*B*n_h  (h_t, t = 0..T-1)
   const float* dlv;          // [T][N][B][8]
   const int32_t* act;        // [T][N][B]
   float* ws;                 // [splits][N][HEAD_WS]
 };
-constexpr int HEAD_WS = 64 * 8 + 8 + NMARL_MAX_NBR * NMARL_MAX_NA;
+constexpr int HEAD_WS = 64 * 8 + 8 + NMARL_MAX_NBR * NMARL_MAX_NA;   // per (split, agent): n_h x 8, then the extras
 
+template <int H>
 __global__ void __launch_bounds__(256) head_wgrad_kernel(const __grid_constant__ nmarl_model m,
                                                         const __grid_constant__ HeadK k) {
-  __shared__ float red[4][64][9];
+  // red[part][unit][c]: 256 / H row parts of H units (only H = 64 runs feature-major)
+  constexpr int NPARTS = 256 / H;
+  __shared__ float red[NPARTS][H][9];
   __shared__ float red2[256];
   const int sp = blockIdx.x, i = blockIdx.y;
   const nmarl_agent& ag = m.agent[i];
-  const int tid = threadIdx.x, u = tid & 63, part = tid >> 6;
+  const int tid = threadIdx.x, u = tid & (H - 1), part = tid >> nmarl_log2(H);
   const long R = (long)k.T * k.B;
   long r_begin, r_end;
-  if (k.fm) {
-    // feature-major h ([t][agent][unit][env]): the coalesced direction is env, so a warp covers 32 consecutive envs and
-    // 8 of the 64 units; 8 x 8 accumulators per thread, one shuffle tree over the envs at the end.  (Reading it with
-    // lanes = units touched 32 different 128-byte lines per load: 0.94 ms for 0.5 GB.)
-    const long nb32 = R / 32, per32 = (nb32 + k.splits - 1) / k.splits;
-    const long blk_begin = (long)sp * per32, blk_end = min(nb32, blk_begin + per32);
-    r_begin = blk_begin * 32; r_end = blk_end * 32;
-    const int lane = tid & 31, w = tid >> 5;
-    float a[8][8];
+  if (H == 64 && k.fm) {
+    if constexpr (H == 64) {       // feature-major state exists on the tensor-core path only (n_h = 64)
+      // feature-major h ([t][agent][unit][env]): the coalesced direction is env, so a warp covers 32 consecutive envs and
+      // 8 of the 64 units; 8 x 8 accumulators per thread, one shuffle tree over the envs at the end.  (Reading it with
+      // lanes = units touched 32 different 128-byte lines per load: 0.94 ms for 0.5 GB.)
+      const long nb32 = R / 32, per32 = (nb32 + k.splits - 1) / k.splits;
+      const long blk_begin = (long)sp * per32, blk_end = min(nb32, blk_begin + per32);
+      r_begin = blk_begin * 32; r_end = blk_end * 32;
+      const int lane = tid & 31, w = tid >> 5;
+      float a[8][8];
 #pragma unroll
-    for (int uu = 0; uu < 8; ++uu)
+      for (int uu = 0; uu < 8; ++uu)
 #pragma unroll
-      for (int c = 0; c < 8; ++c) a[uu][c] = 0.f;
-    for (long blk = blk_begin; blk < blk_end; ++blk) {
-      const long r = blk * 32 + lane, t = r / k.B, b = r - t * k.B;
-      const size_t row = ((size_t)t * k.N + i) * k.B + b;
-      const float4 d0 = *reinterpret_cast<const float4*>(k.dlv + row * 8);
-      const float4 d1 = *reinterpret_cast<const float4*>(k.dlv + row * 8 + 4);
-      const float dl[8] = {d0.x, d0.y, d0.z, d0.w, d1.x, d1.y, d1.z, d1.w};
-      const float* hp = k.h1 + (((size_t)t * k.N + i) * NH + 8 * w) * k.B + b;
+        for (int c = 0; c < 8; ++c) a[uu][c] = 0.f;
+      for (long blk = blk_begin; blk < blk_end; ++blk) {
+        const long r = blk * 32 + lane, t = r / k.B, b = r - t * k.B;
+        const size_t row = ((size_t)t * k.N + i) * k.B + b;
+        const float4 d0 = *reinterpret_cast<const float4*>(k.dlv + row * 8);
+        const float4 d1 = *reinterpret_cast<const float4*>(k.dlv + row * 8 + 4);
+        const float dl[8] = {d0.x, d0.y, d0.z, d0.w, d1.x, d1.y, d1.z, d1.w};
+        const float* hp = k.h1 + (((size_t)t * k.N + i) * NH + 8 * w) * k.B + b;
 #pragma unroll
-      for (int uu = 0; uu < 8; ++uu) {
-        const float hv = hp[(size_t)uu * k.B];
+        for (int uu = 0; uu < 8; ++uu) {
+          const float hv = hp[(size_t)uu * k.B];
 #pragma unroll
-        for (int c = 0; c < 8; ++c) a[uu][c] = fmaf(hv, dl[c], a[uu][c]);
+          for (int c = 0; c < 8; ++c) a[uu][c] = fmaf(hv, dl[c], a[uu][c]);
+        }
       }
+#pragma unroll
+      for (int uu = 0; uu < 8; ++uu)
+#pragma unroll
+        for (int c = 0; c < 8; ++c) {
+          float x = a[uu][c];
+          for (int o = 16; o > 0; o >>= 1) x += __shfl_xor_sync(0xffffffffu, x, o);
+          if (lane == 0) { red[0][8 * w + uu][c] = x; red[1][8 * w + uu][c] = 0.f; red[2][8 * w + uu][c] = 0.f; red[3][8 * w + uu][c] = 0.f; }
+        }
     }
-#pragma unroll
-    for (int uu = 0; uu < 8; ++uu)
-#pragma unroll
-      for (int c = 0; c < 8; ++c) {
-        float x = a[uu][c];
-        for (int o = 16; o > 0; o >>= 1) x += __shfl_xor_sync(0xffffffffu, x, o);
-        if (lane == 0) { red[0][8 * w + uu][c] = x; red[1][8 * w + uu][c] = 0.f; red[2][8 * w + uu][c] = 0.f; red[3][8 * w + uu][c] = 0.f; }
-      }
   } else {
   const long per = (R + k.splits - 1) / k.splits;
   r_begin = (long)sp * per; r_end = min(R, r_begin + per);
   float acc[8];
 #pragma unroll
   for (int c = 0; c < 8; ++c) acc[c] = 0.f;
-  for (long r = r_begin + part; r < r_end; r += 4) {
+  for (long r = r_begin + part; r < r_end; r += NPARTS) {
     const long t = r / k.B, b = r - t * k.B;
     const size_t row = ((size_t)t * k.N + i) * k.B + b;
-    const float hv = k.h1[row * NH + u];
+    const float hv = k.h1[row * H + u];
     const float4 d0 = *reinterpret_cast<const float4*>(k.dlv + row * 8);
     const float4 d1 = *reinterpret_cast<const float4*>(k.dlv + row * 8 + 4);
     acc[0] = fmaf(hv, d0.x, acc[0]); acc[1] = fmaf(hv, d0.y, acc[1]); acc[2] = fmaf(hv, d0.z, acc[2]); acc[3] = fmaf(hv, d0.w, acc[3]);
@@ -578,11 +619,14 @@ __global__ void __launch_bounds__(256) head_wgrad_kernel(const __grid_constant__
   red2[tid] = extra;
   __syncthreads();
   float* w = k.ws + ((size_t)sp * k.N + i) * HEAD_WS;
-  for (int e = tid; e < 64 * 8; e += 256) {
+  for (int e = tid; e < H * 8; e += 256) {
     const int uu = e >> 3, c = e & 7;
-    w[e] = ((red[0][uu][c] + red[1][uu][c]) + red[2][uu][c]) + red[3][uu][c];
+    float x = red[0][uu][c];
+#pragma unroll
+    for (int p = 1; p < NPARTS; ++p) x += red[p][uu][c];
+    w[e] = x;
   }
-  if (tid < n_extra) w[64 * 8 + tid] = red2[tid];
+  if (tid < n_extra) w[H * 8 + tid] = red2[tid];
 }
 
 struct HeadRedK { int N, splits, n_a; const float* ws; float* grads; };
@@ -590,19 +634,19 @@ struct HeadRedK { int N, splits, n_a; const float* ws; float* grads; };
 __global__ void head_reduce_kernel(const __grid_constant__ nmarl_model m, const __grid_constant__ HeadRedK k) {
   const int i = blockIdx.x;
   const nmarl_agent& ag = m.agent[i];
-  const int n_extra = 8 + ag.n_nbr * k.n_a;
-  for (int e = threadIdx.x; e < 64 * 8 + n_extra; e += blockDim.x) {
+  const int n_extra = 8 + ag.n_nbr * k.n_a, H = nmarl_n_h(m);
+  for (int e = threadIdx.x; e < H * 8 + n_extra; e += blockDim.x) {
     float s = 0.f;
     for (int sp = 0; sp < k.splits; ++sp) s += k.ws[((size_t)sp * k.N + i) * HEAD_WS + e];
-    if (e < 64 * 8) {
+    if (e < H * 8) {
       const int u = e >> 3, c = e & 7;
       if (c < k.n_a) k.grads[ag.o_pi_w + u * k.n_a + c] = s;
       else if (c == k.n_a) k.grads[ag.o_v_w + u] = s;
     } else {
-      const int x = e - 64 * 8;
+      const int x = e - H * 8;
       if (x < k.n_a) k.grads[ag.o_pi_b + x] = s;
       else if (x == k.n_a) k.grads[ag.o_v_b] = s;
-      else if (x >= 8) k.grads[ag.o_v_w + NH + (x - 8)] = s;
+      else if (x >= 8) k.grads[ag.o_v_w + H + (x - 8)] = s;
     }
   }
 }
@@ -660,6 +704,7 @@ struct HeadFwdK {                 // pointers are for step 0; t = t0 + blockIdx.
   float loss_scale, v_coef, e_coef;
 };
 
+template <int H>
 __global__ void __launch_bounds__(128) train_heads_kernel(const __grid_constant__ nmarl_model m, const __grid_constant__ HeadFwdK k) {
   __shared__ float red[3][4];
   const int i = blockIdx.y, b = blockIdx.x * 128 + threadIdx.x, B = k.B, t = k.t0 + blockIdx.z;
@@ -675,13 +720,13 @@ __global__ void __launch_bounds__(128) train_heads_kernel(const __grid_constant_
     for (int cc = 0; cc < NMARL_MAX_NA; ++cc) logit[cc] = 0.f;
     float v = 0.f;
 #pragma unroll 4
-    for (int q = 0; q < NH / 4; ++q) {
+    for (int q = 0; q < H / 4; ++q) {
       float4 h4;
       if (k.fm) {
-        const float* hp = k.h1 + ((tb / B + i) * NH + 4 * q) * (size_t)B + b;      // [t][agent][unit][env]
+        const float* hp = k.h1 + ((tb / B + i) * H + 4 * q) * (size_t)B + b;      // [t][agent][unit][env]
         h4 = make_float4(hp[0], hp[(size_t)B], hp[2 * (size_t)B], hp[3 * (size_t)B]);
       } else {
-        h4 = *reinterpret_cast<const float4*>(k.h1 + row * NH + 4 * q);
+        h4 = *reinterpret_cast<const float4*>(k.h1 + row * H + 4 * q);
       }
       const float4 vw = __ldg(reinterpret_cast<const float4*>(P + ag.o_v_w) + q);
 #pragma unroll
@@ -711,7 +756,7 @@ __global__ void __launch_bounds__(128) train_heads_kernel(const __grid_constant_
       if (cc < n_a) { pi[cc] = expf(logit[cc] - mx); se += pi[cc]; } else pi[cc] = 0.f;
 #pragma unroll
     for (int cc = 0; cc < NMARL_MAX_NA; ++cc) if (cc < n_a) pi[cc] = pi[cc] / se;
-    for (int s = 0; s < ag.n_nbr; ++s) v += __ldg(P + ag.o_v_w + NH + s * n_a + k.act[tb + (size_t)ag.nbr[s] * B + b]);
+    for (int s = 0; s < ag.n_nbr; ++s) v += __ldg(P + ag.o_v_w + H + s * n_a + k.act[tb + (size_t)ag.nbr[s] * B + b]);
     v += __ldg(P + ag.o_v_b);
     const int act = k.act[row];
     const float R = k.Rs[row], Adv = k.Advs[row], cs = k.loss_scale;
@@ -756,20 +801,43 @@ __global__ void __launch_bounds__(128) train_heads_kernel(const __grid_constant_
   }
 }
 
-constexpr int BWD_BM = 64, BWD_TY = 16;
+constexpr int BWD_BM = 64;
 
-template <int VAR>
+template <int VAR, int H>
 int launch_bwd(const nmarl_model* m, const BwdK& k, cudaStream_t st) {
-  constexpr int NGRP = (VAR == NMARL_NC) ? 4 : 2;
-  auto kern = cell_bwd_kernel<VAR, BWD_BM, BWD_TY>;
-  const size_t smem = ((size_t)BWD_BM * (NG + 4) + 2 * 16 * 64 * NGRP) * sizeof(float);
+  constexpr int NGRP = (VAR == NMARL_NC) ? 4 : 2, TY = nmarl_ffma_ty(H);
+  auto kern = cell_bwd_kernel<VAR, BWD_BM, TY, H>;
+  const size_t smem = ((size_t)BWD_BM * (4 * H + 4) + 2 * 16 * H * NGRP) * sizeof(float);
   static bool configured = false;
   if (!configured) {
     NMARL_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     configured = true;
   }
   dim3 grid((k.B + BWD_BM - 1) / BWD_BM, m->n_agent);
-  kern<<<grid, 16 * BWD_TY, smem, st>>>(*m, k);
+  kern<<<grid, H / 4 * TY, smem, st>>>(*m, k);
+  NMARL_LAUNCH_CHECK();
+  return 0;
+}
+
+template <int VAR>
+int launch_bwd_width(const nmarl_model* m, const BwdK& k, cudaStream_t st) {
+  switch (nmarl_n_h(*m)) {
+    case 16: return launch_bwd<VAR, 16>(m, k, st);
+    case 32: return launch_bwd<VAR, 32>(m, k, st);
+    case 64: return launch_bwd<VAR, 64>(m, k, st);
+  }
+  nmarl_set_error("n_h %d has no FFMA kernel", nmarl_n_h(*m));
+  return 1;
+}
+
+int launch_dial_msg_bwd(const nmarl_model* m, int B, const float* wt, const float* msg_t, const float* dmsg, float* sv_dmp,
+                        float* dh_rec, cudaStream_t st) {
+  dim3 grid((B + 63) / 64, m->n_agent);
+  switch (nmarl_n_h(*m)) {
+    case 16: dial_msg_bwd_kernel<64, nmarl_ffma_ty(16), 16><<<grid, 256, 0, st>>>(*m, B, wt, msg_t, dmsg, sv_dmp, dh_rec); break;
+    case 32: dial_msg_bwd_kernel<64, nmarl_ffma_ty(32), 32><<<grid, 256, 0, st>>>(*m, B, wt, msg_t, dmsg, sv_dmp, dh_rec); break;
+    default: dial_msg_bwd_kernel<64, nmarl_ffma_ty(64), 64><<<grid, 256, 0, st>>>(*m, B, wt, msg_t, dmsg, sv_dmp, dh_rec); break;
+  }
   NMARL_LAUNCH_CHECK();
   return 0;
 }
@@ -788,7 +856,21 @@ int head_splits(long R) {
   return (int)s;
 }
 
-int run_wgrad(const nmarl_model* m, const nmarl_bwd_args* a, int ngrp, const float* A, int lda, int a_col0,
+template <int ND>
+int launch_wgrad(const WgK& k, dim3 grid, cudaStream_t st) {
+  const size_t smem = (size_t)(2 * 32 * 64 + 2 * 32 * ND) * sizeof(float);
+  static bool configured = false;     // per instantiation
+  if (!configured) {
+    NMARL_CUDA(cudaFuncSetAttribute(wgrad_kernel<ND>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    configured = true;
+  }
+  wgrad_kernel<ND><<<grid, 256, smem, st>>>(k);
+  NMARL_LAUNCH_CHECK();
+  return 0;
+}
+
+// nd: output columns (4 * n_h for the gate GEMM, n_h for the encoders and DIAL's message fc)
+int run_wgrad(const nmarl_model* m, const nmarl_bwd_args* a, int nd, const float* A, int lda, int a_col0,
               const float* D, int ldd, int d_col0, const int* Ka, const int* o_w, const int* o_b, cudaStream_t st) {
   WgK k{};
   k.N = m->n_agent; k.B = a->B; k.T = a->T;
@@ -797,18 +879,18 @@ int run_wgrad(const nmarl_model* m, const nmarl_bwd_args* a, int ngrp, const flo
   int kmax = 0;
   for (int i = 0; i < m->n_agent; ++i) { k.Ka[i] = Ka[i]; kmax = Ka[i] > kmax ? Ka[i] : kmax; }
   k.ka_max = kmax; k.ws = a->ws;
-  const int nd = 64 * ngrp;
   NMARL_CHECK((int64_t)k.splits * k.N * (kmax + 1) * nd <= a->ws_floats, "wgrad: workspace too small");
   dim3 grid(k.splits, kmax > 0 ? (kmax + 63) / 64 : 1, m->n_agent);     // kmax == 0: the bias rows only
-  const size_t smem = (size_t)(2 * 32 * 64 + 2 * 32 * nd) * sizeof(float);
-  static bool configured = false;
-  if (!configured) {
-    NMARL_CUDA(cudaFuncSetAttribute(wgrad_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)((2 * 32 * 64 + 2 * 32 * 256) * sizeof(float))));
-    configured = true;
+  int rc = 1;
+  switch (nd) {
+    case 16: rc = launch_wgrad<16>(k, grid, st); break;
+    case 32: rc = launch_wgrad<32>(k, grid, st); break;
+    case 64: rc = launch_wgrad<64>(k, grid, st); break;
+    case 128: rc = launch_wgrad<128>(k, grid, st); break;
+    case 256: rc = launch_wgrad<256>(k, grid, st); break;
+    default: nmarl_set_error("wgrad: no kernel for %d columns", nd);
   }
-  if (ngrp == 4) wgrad_kernel<4><<<grid, 256, smem, st>>>(k);
-  else wgrad_kernel<1><<<grid, 256, smem, st>>>(k);
-  NMARL_LAUNCH_CHECK();
+  if (rc) return rc;
   WgRedK r{};
   r.N = k.N; r.splits = k.splits; r.ka_max = kmax; r.nd = nd; r.ws = a->ws; r.grads = a->grads;
   for (int i = 0; i < m->n_agent; ++i) { r.Ka[i] = Ka[i]; r.o_w[i] = o_w[i]; r.o_b[i] = o_b[i]; }
@@ -829,7 +911,7 @@ int check_bwd_args(const nmarl_model* m, const nmarl_bwd_args* a) {
   NMARL_CHECK(m->variant == NMARL_IA2C || a->dmsg, "a2c_backward: dmsg buffer required");
   NMARL_CHECK((m->variant != NMARL_IC3 && m->variant != NMARL_DIAL) || a->sv_enc, "a2c_backward: sv_enc required");
   NMARL_CHECK(m->variant != NMARL_DIAL || (a->msg_seq && a->sv_dmp), "a2c_backward: DIAL buffers required");
-  NMARL_CHECK(!a->state_fm || (m->variant != NMARL_DIAL && a->wpack != nullptr && a->B % 128 == 0),
+  NMARL_CHECK(!a->state_fm || (m->variant != NMARL_DIAL && a->wpack != nullptr && a->B % 128 == 0 && nmarl_n_h(*m) == NMARL_NH),
               "a2c_backward: feature-major state needs the tensor-core path (and is not implemented for DIAL)");
   NMARL_CHECK((m->variant != NMARL_NC && m->variant != NMARL_DIAL) || a->fp, "a2c_backward: fp required");
   return 0;
@@ -859,9 +941,9 @@ int nmarl_launch_transposes(const nmarl_model* m, int jobs, const float* params,
 extern "C" int nmarl_loss_tiles(const nmarl_model* m, int B) { (void)m; return nmarl_fwd_tiles(B); }
 
 extern "C" int64_t nmarl_ws_floats(const nmarl_model* m, int B, int T) {
-  const int splits = wgrad_splits((long)B * T);
-  int64_t gate = (int64_t)splits * m->n_agent * (m->s_dim + NH + 1) * NG;
-  int64_t enc = (int64_t)splits * m->n_agent * (m->km_pad + m->kx_pad + 1) * NH;
+  const int splits = wgrad_splits((long)B * T), H = nmarl_n_h(*m);
+  int64_t gate = (int64_t)splits * m->n_agent * (m->s_dim + H + 1) * (4 * H);
+  int64_t enc = (int64_t)splits * m->n_agent * (m->km_pad + m->kx_pad + 1) * H;
   int64_t head = (int64_t)head_splits((long)B * T) * m->n_agent * HEAD_WS;
   int64_t r = gate > enc ? gate : enc;
   r = r > head ? r : head;
@@ -887,7 +969,7 @@ extern "C" int nmarl_nstep_return_adv(int n_agent, int B, int T, int NR, const d
 extern "C" int nmarl_a2c_train_forward(const nmarl_model* m, const nmarl_bwd_args* a, void* stream) {
   if (check_bwd_args(m, a)) return 1;
   cudaStream_t st = (cudaStream_t)stream;
-  const int N = m->n_agent, B = a->B, T = a->T;
+  const int N = m->n_agent, B = a->B, T = a->T, H = nmarl_n_h(*m);
   const size_t nb = (size_t)N * B;
   const int LDI = m->kx_pad + m->kp_pad + m->km_pad;
   const int tiles = nmarl_fwd_tiles(B);
@@ -898,14 +980,14 @@ extern "C" int nmarl_a2c_train_forward(const nmarl_model* m, const nmarl_bwd_arg
     f.obs = a->obs + (size_t)t * nb * m->obs_stride;
     f.fp = a->fp ? a->fp + (size_t)t * nb * m->n_a : nullptr;
     f.done = a->done_pre + (size_t)t * B;
-    f.c_in = a->c_seq + (size_t)t * nb * NH;       f.h_in = a->h_seq + (size_t)t * nb * NH;
-    f.c_out = a->c_seq + (size_t)(t + 1) * nb * NH; f.h_out = a->h_seq + (size_t)(t + 1) * nb * NH;
-    if (m->variant == NMARL_DIAL) { f.msg_in = a->msg_seq + (size_t)t * nb * NH; f.msg_out = a->msg_seq + (size_t)(t + 1) * nb * NH; }
+    f.c_in = a->c_seq + (size_t)t * nb * H;       f.h_in = a->h_seq + (size_t)t * nb * H;
+    f.c_out = a->c_seq + (size_t)(t + 1) * nb * H; f.h_out = a->h_seq + (size_t)(t + 1) * nb * H;
+    if (m->variant == NMARL_DIAL) { f.msg_in = a->msg_seq + (size_t)t * nb * H; f.msg_out = a->msg_seq + (size_t)(t + 1) * nb * H; }
     f.act_in = a->act + (size_t)t * nb;
     f.wpack = a->wpack; f.tc_err = a->tc_err; f.state_fm = a->state_fm;
     int rc = nmarl_launch_train_fwd(m, &f, a->Rs + (size_t)t * nb, a->Advs + (size_t)t * nb,
-                                    a->sv_xin + (size_t)t * nb * LDI, a->sv_sh + (size_t)t * nb * (m->s_dim + NH),
-                                    a->sv_gates + (size_t)t * nb * NG, a->sv_enc ? a->sv_enc + (size_t)t * nb * 128 : nullptr,
+                                    a->sv_xin + (size_t)t * nb * LDI, a->sv_sh + (size_t)t * nb * (m->s_dim + H),
+                                    a->sv_gates + (size_t)t * nb * (4 * H), a->sv_enc ? a->sv_enc + (size_t)t * nb * (2 * H) : nullptr,
                                     a->sv_dlv + (size_t)t * nb * 8, a->loss_part + (size_t)t * N * tiles * 4, scale,
                                     a->v_coef, a->e_coef, st);
     if (rc) return rc;
@@ -920,11 +1002,16 @@ static int launch_train_heads(const nmarl_model* m, const nmarl_bwd_args* a, int
   const size_t nb = (size_t)N * B;
   HeadFwdK k{};
   k.B = B; k.N = N; k.loss_tiles = nmarl_fwd_tiles(B); k.params = a->params; k.fm = a->state_fm; k.t0 = t0;
-  k.h1 = a->h_seq + nb * NH;                                  // h after step t = h_seq[t + 1]
+  k.h1 = a->h_seq + nb * nmarl_n_h(*m);                              // h after step t = h_seq[t + 1]
   k.act = a->act; k.Rs = a->Rs; k.Advs = a->Advs;
   k.sv_dlv = a->sv_dlv; k.loss_part = a->loss_part;
   k.loss_scale = 1.0f / ((float)T * (float)a->B_total); k.v_coef = a->v_coef; k.e_coef = a->e_coef;
-  train_heads_kernel<<<dim3((B + 127) / 128, N, nt), 128, 0, st>>>(*m, k);
+  const dim3 grid((B + 127) / 128, N, nt);
+  switch (nmarl_n_h(*m)) {
+    case 16: train_heads_kernel<16><<<grid, 128, 0, st>>>(*m, k); break;
+    case 32: train_heads_kernel<32><<<grid, 128, 0, st>>>(*m, k); break;
+    default: train_heads_kernel<64><<<grid, 128, 0, st>>>(*m, k); break;
+  }
   NMARL_LAUNCH_CHECK();
   return 0;
 }
@@ -937,14 +1024,15 @@ extern "C" int nmarl_a2c_train_heads(const nmarl_model* m, const nmarl_bwd_args*
 extern "C" int nmarl_a2c_bptt(const nmarl_model* m, const nmarl_bwd_args* a, void* stream) {
   if (check_bwd_args(m, a)) return 1;
   cudaStream_t st = (cudaStream_t)stream;
-  const int N = m->n_agent, B = a->B, T = a->T, SD = m->s_dim;
+  const int N = m->n_agent, B = a->B, T = a->T, SD = m->s_dim, H = nmarl_n_h(*m);
   const size_t nb = (size_t)N * B;
   // 0. gradients of padding slots stay zero
   NMARL_CUDA(cudaMemsetAsync(a->grads, 0, (size_t)m->n_param * sizeof(float), st));
   // 1. transposed weights for the FFMA backward kernels and DIAL's message-gradient kernel (the tensor-core cell
   //    kernels read their own packed transposed operands, refreshed by nmarl_pack_weights)
   //    One launch covers every agent.
-  const bool tc_path = (a->wpack != nullptr && B % 128 == 0 && m->kx_pad <= 32 && m->kp_pad <= 32);
+  // tensor cores: whole 128-env tiles, narrow encoders and the width the wgmma kernels are built for (NMARL_NH)
+  const bool tc_path = (a->wpack != nullptr && B % 128 == 0 && m->kx_pad <= 32 && m->kp_pad <= 32 && H == NMARL_NH);
   if (!tc_path || m->variant == NMARL_DIAL) {
     const int jobs = NMARL_TJ_WXH | (m->variant != NMARL_IA2C ? NMARL_TJ_MSG : 0) | (m->variant == NMARL_DIAL ? NMARL_TJ_MFC : 0);
     if (nmarl_launch_transposes(m, jobs, a->params, a->wt, st)) return 1;
@@ -971,9 +1059,13 @@ extern "C" int nmarl_a2c_bptt(const nmarl_model* m, const nmarl_bwd_args* a, voi
   {
     HeadK h{};
     h.N = N; h.B = B; h.T = T; h.splits = head_splits((long)B * T); h.n_a = m->n_a; h.fm = a->state_fm;
-    h.h1 = a->h_seq + nb * NH; h.dlv = a->sv_dlv; h.act = a->act; h.ws = a->ws;
+    h.h1 = a->h_seq + nb * H; h.dlv = a->sv_dlv; h.act = a->act; h.ws = a->ws;
     NMARL_CHECK((int64_t)h.splits * N * HEAD_WS <= a->ws_floats, "head wgrad: workspace too small");
-    head_wgrad_kernel<<<dim3(h.splits, N), 256, 0, side>>>(*m, h);
+    switch (H) {
+      case 16: head_wgrad_kernel<16><<<dim3(h.splits, N), 256, 0, side>>>(*m, h); break;
+      case 32: head_wgrad_kernel<32><<<dim3(h.splits, N), 256, 0, side>>>(*m, h); break;
+      default: head_wgrad_kernel<64><<<dim3(h.splits, N), 256, 0, side>>>(*m, h); break;
+    }
     NMARL_LAUNCH_CHECK();
     HeadRedK r{N, h.splits, m->n_a, a->ws, a->grads};
     head_reduce_kernel<<<N, 256, 0, side>>>(*m, r);
@@ -987,25 +1079,25 @@ extern "C" int nmarl_a2c_bptt(const nmarl_model* m, const nmarl_bwd_args* a, voi
     k.B = B; k.t = t; k.has_next = (t < T - 1);
     k.params = a->params; k.wt = a->wt;
     k.done_pre = a->done_pre + (size_t)t * B;
-    k.sv_gates = a->sv_gates + (size_t)t * nb * NG;
-    k.sv_sh = a->sv_sh + (size_t)t * nb * (SD + NH);
-    k.sv_enc = a->sv_enc ? a->sv_enc + (size_t)t * nb * 128 : nullptr;
+    k.sv_gates = a->sv_gates + (size_t)t * nb * (4 * H);
+    k.sv_sh = a->sv_sh + (size_t)t * nb * (SD + H);
+    k.sv_enc = a->sv_enc ? a->sv_enc + (size_t)t * nb * (2 * H) : nullptr;
     k.sv_dlv = a->sv_dlv + (size_t)t * nb * 8;
-    k.c_prev = a->c_seq + (size_t)t * nb * NH;
-    k.c_cur = a->c_seq + (size_t)(t + 1) * nb * NH;
+    k.c_prev = a->c_seq + (size_t)t * nb * H;
+    k.c_cur = a->c_seq + (size_t)(t + 1) * nb * H;
     const int pin = (t + 1) & 1, pout = t & 1;
-    k.dh_in = a->dh_rec + (size_t)pin * nb * NH;  k.dh_out = a->dh_rec + (size_t)pout * nb * NH;
-    k.dc_in = a->dc_rec + (size_t)pin * nb * NH;  k.dc_out = a->dc_rec + (size_t)pout * nb * NH;
+    k.dh_in = a->dh_rec + (size_t)pin * nb * H;  k.dh_out = a->dh_rec + (size_t)pout * nb * H;
+    k.dc_in = a->dc_rec + (size_t)pin * nb * H;  k.dc_out = a->dc_rec + (size_t)pout * nb * H;
     if (a->dmsg) {
-      k.dmsg_in = a->dmsg + (size_t)pin * nb * NMARL_MAX_NBR * NH;
-      k.dmsg_out = a->dmsg + (size_t)pout * nb * NMARL_MAX_NBR * NH;
+      k.dmsg_in = a->dmsg + (size_t)pin * nb * NMARL_MAX_NBR * H;
+      k.dmsg_out = a->dmsg + (size_t)pout * nb * NMARL_MAX_NBR * H;
     }
-    k.sv_dpre = a->sv_dpre + (size_t)t * nb * 192;
+    k.sv_dpre = a->sv_dpre + (size_t)t * nb * (3 * H);
     k.wpack = a->wpack; k.tc_err = a->tc_err; k.state_fm = a->state_fm;
     k.raw_tiles = raw_tiles;
-    const bool use_tc = (a->wpack != nullptr && B % 128 == 0 && m->kx_pad <= 32 && m->kp_pad <= 32);
+    const bool use_tc = tc_path;
     // tensor-core path: sv_dz holds the gate-bias partial sums of every 32 env rows [T][N][B/32][256]; FFMA path: dz [T][N][B][256]
-    k.sv_dz = use_tc ? a->sv_dz + (size_t)t * N * (B / 32) * NG : a->sv_dz + (size_t)t * nb * NG;
+    k.sv_dz = use_tc ? a->sv_dz + (size_t)t * N * (B / 32) * (4 * H) : a->sv_dz + (size_t)t * nb * (4 * H);
     k.dzT = (use_tc && a->sv_dzT) ? a->sv_dzT + (size_t)t * N * (B / 32) * (2 * 256 * 32) : nullptr;
     k.ndp = nmarl_tc_ndp(m);
     k.dpT = (use_tc && a->sv_dpT) ? a->sv_dpT + (size_t)t * N * (B / 32) * (2 * k.ndp * 32) : nullptr;
@@ -1015,26 +1107,24 @@ extern "C" int nmarl_a2c_bptt(const nmarl_model* m, const nmarl_bwd_args* a, voi
     if (use_tc) rc = nmarl_tc_launch_bwd(m, k, st);
     else
     switch (m->variant) {
-      case NMARL_IA2C: rc = launch_bwd<NMARL_IA2C>(m, k, st); break;
-      case NMARL_NC: rc = launch_bwd<NMARL_NC>(m, k, st); break;
-      case NMARL_IC3: rc = launch_bwd<NMARL_IC3>(m, k, st); break;
-      case NMARL_DIAL: rc = launch_bwd<NMARL_DIAL>(m, k, st); break;
+      case NMARL_IA2C: rc = launch_bwd_width<NMARL_IA2C>(m, k, st); break;
+      case NMARL_NC: rc = launch_bwd_width<NMARL_NC>(m, k, st); break;
+      case NMARL_IC3: rc = launch_bwd_width<NMARL_IC3>(m, k, st); break;
+      case NMARL_DIAL: rc = launch_bwd_width<NMARL_DIAL>(m, k, st); break;
     }
     if (rc) return rc;
     if (a->ev_step) NMARL_CUDA(cudaEventRecord((cudaEvent_t)a->ev_step[2 * t + 1], st));
     NMARL_DBG_SYNC(st, "cell_bwd");
     if (m->variant == NMARL_DIAL) {
-      dim3 grid((B + 63) / 64, N);
-      dial_msg_bwd_kernel<64, 16><<<grid, 256, 0, st>>>(*m, B, a->wt, a->msg_seq + (size_t)t * nb * NH, k.dmsg_out,
-                                                        a->sv_dmp + (size_t)t * nb * NH, k.dh_out);
-      NMARL_LAUNCH_CHECK();
+      if (launch_dial_msg_bwd(m, B, a->wt, a->msg_seq + (size_t)t * nb * H, k.dmsg_out, a->sv_dmp + (size_t)t * nb * H,
+                              k.dh_out, st)) return 1;
     }
   }
   // 3. weight gradients
   NMARL_CUDA(cudaStreamWaitEvent(st, ev_join, 0));
   int Ka[NMARL_MAX_AGENT], ow[NMARL_MAX_AGENT], ob[NMARL_MAX_AGENT];
   const int LDI = m->kx_pad + m->kp_pad + m->km_pad;
-  const bool tc_wg = (a->wpack != nullptr && B % 128 == 0 && m->kx_pad <= 32 && m->kp_pad <= 32);
+  const bool tc_wg = tc_path;
   if (tc_wg) {
     NMARL_CHECK(a->sv_dzT && a->sv_dpT, "a2c_bptt: tensor-core path needs sv_dzT / sv_dpT");
     NMARL_CHECK(nmarl_tc_wgrad_ws_floats(m) <= a->ws_floats, "tc wgrad: workspace too small");
@@ -1047,26 +1137,26 @@ extern "C" int nmarl_a2c_bptt(const nmarl_model* m, const nmarl_bwd_args* a, voi
     NMARL_CUDA(cudaStreamWaitEvent(st, ev_join, 0));
     NMARL_DBG_SYNC(st, "tc_wgrads");
   } else {
-    for (int i = 0; i < N; ++i) { Ka[i] = SD + NH; ow[i] = m->agent[i].o_wxh; ob[i] = m->agent[i].o_b; }
-    if (run_wgrad(m, a, 4, a->sv_sh, SD + NH, 0, a->sv_dz, NG, 0, Ka, ow, ob, st)) return 1;
+    for (int i = 0; i < N; ++i) { Ka[i] = SD + H; ow[i] = m->agent[i].o_wxh; ob[i] = m->agent[i].o_b; }
+    if (run_wgrad(m, a, 4 * H, a->sv_sh, SD + H, 0, a->sv_dz, (4 * H), 0, Ka, ow, ob, st)) return 1;
     for (int i = 0; i < N; ++i) { Ka[i] = m->agent[i].x_nsrc * m->agent[i].x_w; ow[i] = m->agent[i].o_w_ob; ob[i] = m->agent[i].o_b_ob; }
-    if (run_wgrad(m, a, 1, a->sv_xin, LDI, 0, a->sv_dpre, 192, 0, Ka, ow, ob, st)) return 1;
+    if (run_wgrad(m, a, H, a->sv_xin, LDI, 0, a->sv_dpre, 3 * H, 0, Ka, ow, ob, st)) return 1;
     if (m->variant == NMARL_NC) {
       for (int i = 0; i < N; ++i) { Ka[i] = m->agent[i].n_nbr * m->n_a; ow[i] = m->agent[i].o_w_fp; ob[i] = m->agent[i].o_b_fp; }
-      if (run_wgrad(m, a, 1, a->sv_xin, LDI, m->kx_pad, a->sv_dpre, 192, NH, Ka, ow, ob, st)) return 1;
+      if (run_wgrad(m, a, H, a->sv_xin, LDI, m->kx_pad, a->sv_dpre, 3 * H, H, Ka, ow, ob, st)) return 1;
     }
     if (m->variant != NMARL_IA2C) {
       for (int i = 0; i < N; ++i) {
-        Ka[i] = (m->variant == NMARL_IC3) ? NH : m->agent[i].n_nbr * NH;
+        Ka[i] = (m->variant == NMARL_IC3) ? H : m->agent[i].n_nbr * H;
         ow[i] = m->agent[i].o_w_msg; ob[i] = m->agent[i].o_b_msg;
       }
-      if (run_wgrad(m, a, 1, a->sv_xin, LDI, m->kx_pad + m->kp_pad, a->sv_dpre, 192, (m->variant == NMARL_NC) ? 2 * NH : NH,
+      if (run_wgrad(m, a, H, a->sv_xin, LDI, m->kx_pad + m->kp_pad, a->sv_dpre, 3 * H, (m->variant == NMARL_NC) ? 2 * H : H,
                     Ka, ow, ob, st)) return 1;
     }
   }
   if (m->variant == NMARL_DIAL) {
-    for (int i = 0; i < N; ++i) { Ka[i] = NH; ow[i] = m->agent[i].o_mfc_w; ob[i] = m->agent[i].o_mfc_b; }
-    if (run_wgrad(m, a, 1, a->h_seq, NH, 0, a->sv_dmp, NH, 0, Ka, ow, ob, st)) return 1;
+    for (int i = 0; i < N; ++i) { Ka[i] = H; ow[i] = m->agent[i].o_mfc_w; ob[i] = m->agent[i].o_mfc_b; }
+    if (run_wgrad(m, a, H, a->h_seq, H, 0, a->sv_dmp, H, 0, Ka, ow, ob, st)) return 1;
   }
   (void)0;
   return 0;
@@ -1124,9 +1214,9 @@ __global__ void __launch_bounds__(256) consensus_store_kernel(const __grid_const
 extern "C" int nmarl_consensus_update(const nmarl_model* m, float* params, float* scratch, void* stream) {
   if (nmarl_check_model(m)) return 1;
   NMARL_CHECK(params && scratch, "consensus_update: missing buffers");
-  const int n = (m->s_dim + NH) * NG + NG;
+  const int G = 4 * nmarl_n_h(*m), n = (m->s_dim + nmarl_n_h(*m)) * G + G;
   for (int i = 0; i < m->n_agent; ++i)
-    NMARL_CHECK(m->agent[i].o_b == m->agent[i].o_wxh + (m->s_dim + NH) * NG, "consensus_update: LSTM block of agent %d is not contiguous", i);
+    NMARL_CHECK(m->agent[i].o_b == m->agent[i].o_wxh + (m->s_dim + nmarl_n_h(*m)) * G, "consensus_update: LSTM block of agent %d is not contiguous", i);
   cudaStream_t st = (cudaStream_t)stream;
   consensus_mean_kernel<<<dim3(32, m->n_agent), 256, 0, st>>>(*m, params, scratch, n);
   NMARL_LAUNCH_CHECK();

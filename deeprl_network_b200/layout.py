@@ -20,7 +20,10 @@ Two agents reuse another agent's kernels (SURVEY 8 f2):
 
 In the flat buffer every tensor starts on a 16-byte boundary, one agent's tensors are
 contiguous (IA2C clips/optimises per agent) and wx_hid/wh_hid are adjacent so the LSTM gate
-GEMM sees one [s_dim+64, 256] matrix.
+GEMM sees one [s_dim+n_h, 4*n_h] matrix.
+
+Width: num_lstm = n_h in {16, 32, 64}.  The MA2C family and ma2c_cu size every encoder by n_h and ignore num_fc
+(agents/policies.py:192, agents/models.py:103-104); ia2c / ia2c_fp need num_fc == num_lstm.
 """
 import numpy as np
 
@@ -30,7 +33,7 @@ VARIANT_ID = {'ia2c': L.IA2C, 'ma2c_nc': L.NC, 'ma2c_ic3': L.IC3, 'ma2c_dial': L
 PER_AGENT_OPT = ('ia2c', 'ia2c_fp')        # one loss / clip / optimizer per agent (agents/models.py:34-42)
 SCOPE = {'ma2c_nc': 'nc', 'ma2c_ic3': 'ic3', 'ma2c_dial': 'dial'}
 CELL = {'ma2c_nc': 'lstm_comm', 'ma2c_ic3': 'lstm_ic3', 'ma2c_dial': 'lstm_comm'}
-NH = L.NH
+NH = L.NH             # default width; a layout's own width is ModelLayout.n_h
 
 
 def _up4(x):
@@ -51,10 +54,15 @@ class ModelLayout:
         """obs_mode 'gather': the obs buffer holds each agent's OWN features (width base_n_s) and the
         kernel concatenates own + neighbours' rows (what the MA2C graphs do, and equal to the IA2C
         env observation).  'concat' (IA2C API mode): rows are the caller's pre-concatenated obs."""
-        if n_h != NH or n_fc != NH:
-            raise ValueError('kernels are specialised for num_lstm = num_fc = 64 (got %d/%d)' % (n_h, n_fc))
         if variant not in VARIANT_ID:
             raise ValueError('unsupported agent %r (covered: ia2c, ia2c_fp, ma2c_cu, ma2c_nc, ma2c_ic3, ma2c_dial)' % variant)
+        n_h, n_fc = int(n_h), int(n_fc)
+        if n_h not in L.WIDTHS:
+            raise ValueError('num_lstm = %d is not supported (kernels exist for %s)' % (n_h, ', '.join(map(str, L.WIDTHS))))
+        if variant in ('ia2c', 'ia2c_fp') and n_fc != n_h:
+            # the MA2C family and ma2c_cu size their encoders by num_lstm and ignore num_fc, as the reference does
+            raise ValueError('%s needs num_fc == num_lstm (got num_fc = %d, num_lstm = %d)' % (variant, n_fc, n_h))
+        self.n_h = n_h
         self.variant, self.vid = variant, VARIANT_ID[variant]
         mask = np.asarray(neighbor_mask).astype(int)
         N = len(mask)
@@ -90,7 +98,7 @@ class ModelLayout:
         else:
             self.base_n_s = self.n_s_ls[0]
             assert all(x == self.base_n_s for x in self.n_s_ls), 'MA2C agents must share n_s'
-        self.s_dim = 3 * NH if variant in ('ma2c_nc', 'ia2c_fp') else NH
+        self.s_dim = 3 * n_h if variant in ('ma2c_nc', 'ia2c_fp') else n_h
         self._build()
 
     # ------------------------------------------------------------------------------------------
@@ -102,7 +110,7 @@ class ModelLayout:
         return self.base_n_s * (1 + len(self.nbr[i]))
 
     def _build(self):
-        N, n_a, v = self.N, self.n_a, self.variant
+        N, n_a, v, NH = self.N, self.n_a, self.variant, self.n_h
         self.entries = []          # (reference name, offset, shape)
         self.agents_off = []
         off = 0
@@ -207,7 +215,7 @@ class ModelLayout:
 
     def c_model(self):
         m = L.Model()
-        m.variant, m.n_agent, m.n_a, m.s_dim = self.vid, self.N, self.n_a, self.s_dim
+        m.variant, m.n_agent, m.n_a, m.s_dim = self.vid, self.N, self.n_a, self.s_dim       # s_dim carries n_h
         m.obs_stride, m.kx_pad, m.kp_pad, m.km_pad = self.obs_stride, self.kx_pad, self.kp_pad, self.km_pad
         m.n_param, m.n_wt, m.n_wp = self.n_param, self.n_wt, self.n_wp
         m.per_agent_norm = 1 if self.variant in PER_AGENT_OPT else 0
@@ -351,7 +359,7 @@ class HeteroLayout(ModelLayout):
         self._embed()
 
     def _embed(self):
-        v, N, ns_max, na_max = self.variant, self.N, self.base_n_s, self.n_a
+        v, N, ns_max, na_max, NH = self.variant, self.N, self.base_n_s, self.n_a, self.n_h
         pad = {n: (o, s) for n, o, s in self.entries}           # padded tensors of the inner homogeneous layout
         tight, idx = [], {}
 

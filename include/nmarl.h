@@ -32,7 +32,9 @@ extern "C" {
  * stays inside the 32 764-byte kernel-parameter limit of sm_90 with room for each kernel's argument block       */
 #define NMARL_MAX_AGENT 128
 #define NMARL_MAX_NBR   4
-#define NMARL_NH        64      /* LSTM width (num_lstm = num_fc = 64 in every shipped config) */
+/* LSTM width the tensor-core kernels are built for (num_lstm = 64 in every shipped config).  The FP32-FFMA kernels
+ * also run n_h = 16 and 32 (n_h follows from nmarl_model.s_dim); any other model never takes the tensor-core path. */
+#define NMARL_NH        64
 #define NMARL_MAX_NA    8
 
 enum { NMARL_IA2C = 0, NMARL_NC = 1, NMARL_IC3 = 2, NMARL_DIAL = 3 };
@@ -73,7 +75,10 @@ typedef struct {
 
 typedef struct {
   int32_t variant;                       /* NMARL_IA2C / NC / IC3 / DIAL                        */
-  int32_t n_agent, n_a, s_dim;           /* s_dim = 192 (NC) or 64                              */
+  int32_t n_agent, n_a, s_dim;           /* s_dim = 3 * n_h (NC) or n_h, which gives the LSTM     */
+                                         /*   width n_h = num_lstm: 16, 32 or 64 (NMARL_NH, the   */
+                                         /*   only width with tensor-core kernels).  Every "64"   */
+                                         /*   below is n_h, every "256" is 4 * n_h                */
   int32_t obs_stride;                    /* floats per obs row                                  */
   int32_t kx_pad, kp_pad, km_pad;        /* padded (x4) widths of the x~ / p~ / m~ input segments */
   int32_t n_param, n_wt;                 /* flat buffer sizes (floats)                          */
@@ -150,7 +155,8 @@ typedef struct {
   const int32_t* act_in;   /* v-call / train: [N][B] same-step actions                         */
   float* v;                /* v-call: [N][B]                                                   */
   const float* wpack;      /* packed 3xTF32 operands (nmarl_pack_weights) or NULL.  When set and  */
-                           /* B % 128 == 0 the wgmma tensor-core kernel is used, else FP32 FFMA */
+                           /* B % 128 == 0 and n_h == 64 the wgmma tensor-core kernel is used,  */
+                           /* else FP32 FFMA (which ignores wpack)                              */
   int32_t* tc_err;         /* device int: tensor-core pipeline watchdog (0 = ok); may be NULL      */
   /* optional (p-call, tensor-core path only): save the activations BPTT needs while rolling out, so the
    * update can skip the separate training forward (same inputs, same weights => same numbers):         */
@@ -192,8 +198,9 @@ int nmarl_nstep_return_adv(int n_agent, int B, int T, int NR, const double* rewa
  *   h_seq, c_seq [T+1][N][B][64]  (index 0 = states_bw, filled by the caller)
  *   msg_seq      [T+1][N][B][64]  (DIAL; index 0 filled by nmarl_dial_msg)
  *   sv_xin [T][N][B][kx_pad+kp_pad+km_pad]  sv_sh [T][N][B][s_dim+64]  sv_gates [T][N][B][256]
- *   sv_enc [T][N][B][128] (IC3: 64 used; DIAL: 128)   sv_dlv [T][N][B][8]
- *   sv_dz [T][N][B][256]   sv_dpre [T][N][B][192]   sv_dmp [T][N][B][64] (DIAL)
+ *   sv_enc [T][N][B][2*n_h] (IC3: n_h used; DIAL: 2*n_h)   sv_dlv [T][N][B][8]
+ *   sv_dz [T][N][B][4*n_h]   sv_dpre [T][N][B][3*n_h]   sv_dmp [T][N][B][n_h] (DIAL)
+ *   (the widths written 64 / 256 / 192 in this block are n_h / 4*n_h / 3*n_h; the tensor-core path has n_h = 64)
  *   (tensor-core path: sv_dz = [T][N][B/32][256] gate-bias partial sums per 32 rows, sv_dpre unused)
  *   dh_rec, dc_rec [2][N][B][64]   dmsg [2][N][MAX_NBR][B][64]
  *   wt [n_wt] transposed weights   ws: split-K workspace of ws_floats floats
@@ -260,7 +267,7 @@ int nmarl_clip_rmsprop_step(const nmarl_model* m, float* params, float* grads, f
  * Replaces ConsensusPolicy._consensus_update (agents/policies.py:351-359, 401-426), run after every
  * optimizer step: agent i's LSTM variables (wx, wh, b -- one contiguous block of the flat buffer) become
  * the mean of the blocks of {i} + its neighbours (ascending index), all read BEFORE any is written.
- *   scratch: device float [n_agent * ((s_dim + 64) * 256 + 256)]                                         */
+ *   scratch: device float [n_agent * ((s_dim + n_h) * 4*n_h + 4*n_h)]                                         */
 int nmarl_consensus_update(const nmarl_model* m, float* params, float* scratch, void* stream);
 
 #pragma GCC visibility pop
