@@ -79,7 +79,7 @@ EXPORTS = ['nmarl_last_error', 'nmarl_version', 'nmarl_create', 'nmarl_destroy',
            'nmarl_cacc_reset', 'nmarl_cacc_step', 'nmarl_pack_weights', 'nmarl_policy_step_p', 'nmarl_policy_step_v', 'nmarl_dial_msg',
            'nmarl_rng_advance', 'nmarl_nstep_return_adv', 'nmarl_loss_tiles', 'nmarl_ws_floats',
            'nmarl_a2c_backward', 'nmarl_a2c_train_forward', 'nmarl_a2c_bptt', 'nmarl_a2c_train_heads',
-           'nmarl_clip_rmsprop_step', 'nmarl_consensus_update']
+           'nmarl_clip_rmsprop_step', 'nmarl_consensus_update', 'nmarl_eval_record']
 
 
 def lib():
@@ -110,6 +110,7 @@ def lib():
         getattr(L, fn).argtypes = [C.POINTER(Model), C.POINTER(BwdArgs), P]
     L.nmarl_clip_rmsprop_step.argtypes = [C.POINTER(Model), P, P, P, P, F, F, F, P, P, P]
     L.nmarl_consensus_update.argtypes = [C.POINTER(Model), P, P, P]
+    L.nmarl_eval_record.argtypes = [I, I, I, I, P, P, P, P, P, P, P, P, P, P, P, P, P, P]
     assert L.nmarl_sizeof_model() == C.sizeof(Model), 'nmarl_model layout mismatch'
     assert L.nmarl_sizeof_agent() == C.sizeof(Agent), 'nmarl_agent layout mismatch'
     assert L.nmarl_sizeof_cacc_cfg() == C.sizeof(CaccCfg), 'nmarl_cacc_cfg layout mismatch'

@@ -20,8 +20,10 @@ from .. import _lib as L
 
 class PolicyEngine:
     def __init__(self, layout, n_env, n_step, hp, flat_params=None, device=None, rng_seed=0,
-                 distance_mask=None, coop_gamma=-1.0, group=None, use_tc=None):
-        """hp: dict(v_coef, e_coef, max_grad_norm, alpha, epsilon, gamma, reward_norm, reward_clip)."""
+                 distance_mask=None, coop_gamma=-1.0, group=None, use_tc=None, shared_params=None):
+        """hp: dict(v_coef, e_coef, max_grad_norm, alpha, epsilon, gamma, reward_norm, reward_clip).
+        shared_params: another engine's parameter tensor, read in place instead of a copy of flat_params (an
+        evaluation engine that follows the trained weights; it must not be trained itself)."""
         L.require_cuda()
         self.layout, self.B, self.T, self.hp = layout, int(n_env), int(n_step), dict(hp)
         self.N, self.n_a, self.n_h = layout.N, layout.n_a, layout.n_h
@@ -35,9 +37,13 @@ class PolicyEngine:
         self.variant = {'ma2c_cu': 'ia2c', 'ia2c_fp': 'ma2c_nc'}.get(layout.variant, layout.variant)
         dev, N, B, T = self.device, self.N, self.B, self.T
         f32 = dict(dtype=torch.float32, device=dev)
-        if flat_params is None:
-            flat_params = layout.init_flat()
-        self.params = torch.as_tensor(np.asarray(flat_params, dtype=np.float32)).to(dev).contiguous()
+        if shared_params is not None:
+            assert shared_params.dtype == torch.float32 and shared_params.device == dev and shared_params.is_contiguous()
+            self.params = shared_params
+        else:
+            if flat_params is None:
+                flat_params = layout.init_flat()
+            self.params = torch.as_tensor(np.asarray(flat_params, dtype=np.float32)).to(dev).contiguous()
         assert self.params.numel() == layout.n_param
         self.grads = torch.zeros(layout.n_param, **f32)
         self.ms = torch.ones(layout.n_param, **f32)             # TF RMSProp slot starts at 1

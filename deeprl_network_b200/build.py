@@ -13,7 +13,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, 'csrc')
 LIB = os.path.join(HERE, 'libnmarl.so')
-SOURCES = [('api.cu', []), ('env.cu', ['--fmad=false']), ('cell_fwd.cu', []), ('train.cu', []), ('tc_gemm.cu', []), ('tc_cell.cu', []), ('tc_bwd.cu', []), ('tc_wgrad.cu', [])]
+SOURCES = [('api.cu', []), ('env.cu', ['--fmad=false']), ('cell_fwd.cu', []), ('train.cu', []), ('tc_gemm.cu', []), ('tc_cell.cu', []), ('tc_bwd.cu', []), ('tc_wgrad.cu', []), ('eval.cu', [])]
 ARCH = ['-gencode', 'arch=compute_90a,code=sm_90a']
 COMMON = ['-O3', '-lineinfo', '-std=c++17', '-Xcompiler', '-fPIC', '-Xcompiler', '-fvisibility=hidden']
 

@@ -13,7 +13,8 @@ void nmarl_set_error(const char* fmt, ...) {
 }
 
 extern "C" const char* nmarl_last_error(void) { return g_err; }
-extern "C" int nmarl_version(void) { return 102; }     // 101: NMARL_MAX_AGENT 32 -> 128; 102: n_h = 16 / 32 (s_dim)
+// 101: NMARL_MAX_AGENT 32 -> 128; 102: n_h = 16 / 32 (s_dim); 103: nmarl_eval_record
+extern "C" int nmarl_version(void) { return 103; }
 extern "C" int nmarl_sizeof_model(void) { return (int)sizeof(nmarl_model); }
 extern "C" int nmarl_sizeof_agent(void) { return (int)sizeof(nmarl_agent); }
 extern "C" int nmarl_sizeof_cacc_cfg(void) { return (int)sizeof(nmarl_cacc_cfg); }

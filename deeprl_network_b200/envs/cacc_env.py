@@ -251,34 +251,50 @@ class CACCEnv:
         self._trace.append(torch.stack([self.hs[:, 0], self.vs[:, 0], self.us[:, 0]]).cpu().numpy())
 
     def _log_control_data(self, action, global_reward):
-        self.control_data.append({'episode': self.cur_episode, 'time_sec': self.t * self.dt, 'step': self.t,
-                                  'action': ','.join(['%d' % a for a in action]), 'reward': global_reward})
+        self.control_data.append(control_record(self.cur_episode, self.t, self.dt, action, global_reward))
 
     def _log_traffic_data(self):
-        import pandas as pd
-        tr = np.array(self._trace)                 # [steps, 3, N]
-        hs, vs, us = tr[:, 0], tr[:, 1], tr[:, 2]
-        df = pd.DataFrame()
-        df['episode'] = np.ones(len(hs)) * self.cur_episode
-        df['time_sec'] = np.arange(len(hs)) * self.dt
-        df['reward'] = np.array(self.rewards)
-        df['lead_headway_m'] = hs[:, 0]
-        df['avg_headway_m'] = np.mean(hs[:, 1:], axis=1)
-        df['std_headway_m'] = np.std(hs[:, 1:], axis=1)
-        df['avg_speed_mps'] = np.mean(vs, axis=1)
-        df['std_speed_mps'] = np.std(vs, axis=1)
-        df['avg_accel_mps2'] = np.mean(us, axis=1)
-        df['std_accel_mps2'] = np.std(us, axis=1)
-        for i in range(self.n_agent):
-            df['headway_%d_m' % (i + 1)] = hs[:, i]
-            df['velocity_%d_mps' % (i + 1)] = vs[:, i]
-            df['accel_%d_mps2' % (i + 1)] = us[:, i]
-        self.traffic_data.append(df)
+        self.traffic_data.append(traffic_frame(self.cur_episode, np.array(self._trace), self.rewards, self.dt))
 
     def output_data(self):
-        import pandas as pd
         if not self.is_record:
             logging.error('Env: no record to output!')
             return
-        pd.DataFrame(self.control_data).to_csv(self.output_path + ('%s_%s_control.csv' % (self.name, self.agent)))
-        pd.concat(self.traffic_data).to_csv(self.output_path + ('%s_%s_traffic.csv' % (self.name, self.agent)))
+        write_records(self.output_path, self.name, self.agent, self.control_data, self.traffic_data)
+
+
+# ---- record formats (envs/cacc_env.py:81-112); shared by CACCEnv and the batched evaluator (utils.py) ---------------
+def control_record(episode, t, dt, action, global_reward):
+    """One row of <scenario>_<agent>_control.csv: step t (1-based) of episode `episode`."""
+    return {'episode': episode, 'time_sec': t * dt, 'step': t, 'action': ','.join(['%d' % a for a in action]),
+            'reward': global_reward}
+
+
+def traffic_frame(episode, tr, rewards, dt):
+    """The rows of <scenario>_<agent>_traffic.csv for one episode.  tr: float64 [steps + 1, 3, N] = (hs, vs, us) of
+    the reset state and of every step; rewards: the steps + 1 global rewards, the reset's 0 first."""
+    import pandas as pd
+    hs, vs, us = tr[:, 0], tr[:, 1], tr[:, 2]
+    df = pd.DataFrame()
+    df['episode'] = np.ones(len(hs)) * episode
+    df['time_sec'] = np.arange(len(hs)) * dt
+    df['reward'] = np.array(rewards)
+    df['lead_headway_m'] = hs[:, 0]
+    df['avg_headway_m'] = np.mean(hs[:, 1:], axis=1)
+    df['std_headway_m'] = np.std(hs[:, 1:], axis=1)
+    df['avg_speed_mps'] = np.mean(vs, axis=1)
+    df['std_speed_mps'] = np.std(vs, axis=1)
+    df['avg_accel_mps2'] = np.mean(us, axis=1)
+    df['std_accel_mps2'] = np.std(us, axis=1)
+    for i in range(tr.shape[2]):
+        df['headway_%d_m' % (i + 1)] = hs[:, i]
+        df['velocity_%d_mps' % (i + 1)] = vs[:, i]
+        df['accel_%d_mps2' % (i + 1)] = us[:, i]
+    return df
+
+
+def write_records(output_path, name, agent, control_data, traffic_data):
+    """control_data: list of control_record rows; traffic_data: list of traffic_frame frames, in episode order."""
+    import pandas as pd
+    pd.DataFrame(control_data).to_csv(output_path + ('%s_%s_control.csv' % (name, agent)))
+    pd.concat(traffic_data).to_csv(output_path + ('%s_%s_traffic.csv' % (name, agent)))

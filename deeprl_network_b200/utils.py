@@ -9,7 +9,8 @@ bootstrap at a non-terminal batch end is one more policy + value call, Q4 the re
 that of a greedy test episode run after every training episode, Q5 only training steps are counted.
 
 ``VecTrainer`` is the batched loop this package adds (n_env parallel episodes, everything device resident,
-optionally one process per GPU with one NCCL gradient all-reduce per update).
+optionally one process per GPU with one NCCL gradient all-reduce per update).  ``BatchedEvaluator`` runs the greedy
+test episodes of many seeds at once on the device and writes what ``Evaluator`` writes, byte for byte.
 """
 import logging
 import pathlib
@@ -18,6 +19,11 @@ import time
 
 import numpy as np
 import torch
+
+from . import _lib as L
+from .agents.engine import PolicyEngine
+from .envs.cacc_env import CACCEnv, control_record, traffic_frame, write_records
+from .layout import ModelLayout
 
 _TEST_MODES = {'no_test': (False, False), 'in_train_test': (True, False),
                'after_train_test': (False, True), 'all_test': (True, True)}
@@ -348,3 +354,167 @@ class VecTrainer:
     def write_csv(self, output_path):
         import pandas as pd
         pd.DataFrame(self.data).to_csv(output_path + 'train_reward.csv')
+
+
+class BatchedEvaluator:
+    """Greedy test episodes of many seeds in one pass on the device: what ``Evaluator`` does one seed at a time.
+
+    Env b of a pass starts from test seed b with the host draws of ``CACCEnv.reset(test_ind=b)``; every step is one
+    greedy p-call (pi goes straight into the next fingerprint slot), one test-mode env step and one
+    ``nmarl_eval_record`` launch, with no host round trip until the pass ends.  The model is a second engine over
+    the trained parameter tensor itself: no weights are copied, and the trained model's states, RNG and buffers are
+    not touched.
+
+    It always runs the FP32-FFMA kernels.  Their per-row arithmetic does not depend on the number of envs and the env
+    step is per env, so every action, and therefore every file, equals the one-env ``Evaluator``'s bit for bit; the
+    tensor-core kernels round differently and would flip near-tie arg-maxes.
+
+    Seeds go through in passes of at most ``max_env`` envs whose records fit in ``record_bytes`` of device memory
+    (DESIGN §4.7).  With ``graph`` the steps of a pass are captured into a CUDA graph on the second pass of a size
+    and replayed from then on.
+    """
+
+    def __init__(self, env_config, model, output_path=None, max_env=4096, record_bytes=2 ** 31, graph=True):
+        self.config, self.model, self.output_path = env_config, model, output_path
+        self.max_env, self.record_bytes, self.use_graph = int(max_env), int(record_bytes), graph
+        self.layout = self._eval_layout(model.layout)
+        self.agent = env_config.get('agent')
+        self._runners = {}
+        self.data = []                     # test_reward.csv records (log_test)
+
+    @staticmethod
+    def _eval_layout(lay):
+        if getattr(lay, 'hetero', False):
+            raise ValueError('batched evaluation runs homogeneous agents (the CACC platoons have them)')
+        if lay.variant == 'ia2c' and lay.obs_mode != 'gather':
+            # device rollouts gather the neighbours' observation rows in the kernel; the one-env model reads the
+            # caller's concatenation.  Both give the kernel the same input row and the same parameter layout.
+            g = ModelLayout('ia2c', lay.n_s_ls, lay.n_a, lay.mask, n_h=lay.n_h, n_fc=lay.n_h, obs_mode='gather')
+            assert g.entries == lay.entries and g.n_param == lay.n_param and g.kx_pad == lay.kx_pad
+            return g
+        return lay
+
+    def chunk_size(self, n_seed):
+        """Envs per pass: at most max_env, and records of at most record_bytes."""
+        lay, T = self.layout, self._episode_len()
+        per_env = (T + 1) * (lay.N * (4 + 3 * 8) + 8)
+        return max(1, min(self.max_env, int(n_seed), self.record_bytes // per_env))
+
+    def _episode_len(self):
+        return int(self.config.getint('episode_length_sec') / self.config.getfloat('control_interval_sec'))
+
+    def _runner(self, E):
+        r = self._runners.get(E)
+        if r is not None:
+            return r
+        src = self.model.engine
+        env = CACCEnv(self.config, n_env=E, device=src.device)
+        env.train_mode = False
+        eng = PolicyEngine(self.layout, E, 1, dict(src.hp), device=src.device, use_tc=False, shared_params=src.params)
+        T, N, dev = env.T, env.n_agent, src.device
+        z = lambda *s, dtype=torch.float64: torch.zeros(*s, dtype=dtype, device=dev)
+        r = dict(env=env, eng=eng, T=T, u01=z(*env.v_init.shape), alive=z(E, dtype=torch.int32),
+                 steps=z(E, dtype=torch.int32), action=z(T + 1, E, N, dtype=torch.int32), reward=z(T + 1, E),
+                 hs=z(T + 1, E, N), vs=z(T + 1, E, N), us=z(T + 1, E, N), graph=None, passes=0)
+        self._runners[E] = r
+        return r
+
+    def _record(self, r, start, done=None):
+        env, eng = r['env'], r['eng']
+        L.check(L.lib().nmarl_eval_record(env.n_agent, env.n_env, r['T'], int(start), L.ptr(eng.act_buf[0]),
+                                          L.ptr(env.greward_dev), L.ptr(done), L.ptr(env.hs), L.ptr(env.vs),
+                                          L.ptr(env.us), L.ptr(r['alive']), L.ptr(r['steps']), L.ptr(r['action']),
+                                          L.ptr(r['reward']), L.ptr(r['hs']), L.ptr(r['vs']), L.ptr(r['us']),
+                                          L.stream()), 'nmarl_eval_record')
+
+    def _steps(self, r):
+        """The T greedy steps of a pass.  Slots 0 / 1 of the engine's buffers take turns as 'now' and 'next'."""
+        env, eng = r['env'], r['eng']
+        for t in range(r['T']):
+            s, n = t & 1, 1 - (t & 1)
+            eng.step_p(eng.obs_buf[s], eng.fp_buf[s], eng.done_buf[s], eng.fp_buf[n], eng.act_buf[0], L.SAMPLE_GREEDY)
+            env.step_device(eng.act_buf[0], obs_out=eng.obs_buf[n], done_out=eng.done_buf[n])   # rewards: env's own
+            self._record(r, False, eng.done_buf[n])
+
+    def _pass(self, seeds):
+        """One greedy episode per seed, all at once -> host arrays (steps [E], action [T+1,E,N], reward [T+1,E],
+        hs / vs / us [T+1,E,N]); episode b holds slots 0..steps[b]."""
+        r = self._runner(len(seeds))
+        env, eng = r['env'], r['eng']
+        u = np.empty(tuple(r['u01'].shape))
+        for b, seed in enumerate(seeds):              # CACCEnv.reset(test_ind): np.random.seed, then one draw per platoon
+            np.random.seed(seed)
+            u[:, b] = [np.random.rand() for _ in range(u.shape[0])]
+        r['u01'].copy_(torch.from_numpy(u))
+        eng.cur = 0                                   # the graph was captured from slot 0
+        eng.reset_states()
+        env.reset_device(u01=r['u01'], obs_out=eng.obs_buf[0], fp_out=eng.fp_buf[0])
+        eng.done_buf[0].fill_(1.0)
+        self._record(r, True)
+        if self.use_graph and r['graph'] is None and r['passes'] > 0:
+            r['graph'] = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(r['graph']):
+                self._steps(r)
+        if r['graph'] is not None:
+            r['graph'].replay()
+        else:
+            self._steps(r)
+        r['passes'] += 1
+        return tuple(r[k].cpu().numpy() for k in ('steps', 'action', 'reward', 'hs', 'vs', 'us'))
+
+    def episodes(self, seeds):
+        """The greedy episode of every seed, in seed order, as split_episodes yields them."""
+        rng = np.random.get_state()                   # the host draws in _pass must not move the caller's stream
+        try:
+            E = self.chunk_size(len(seeds))
+            for c0 in range(0, len(seeds), E):
+                yield from split_episodes(c0, *self._pass(seeds[c0:c0 + E]))
+        finally:
+            np.random.set_state(rng)
+
+    def run(self, seeds):
+        """main.py evaluate: the two record files and the log lines of Evaluator.run for these test seeds."""
+        name = self.config.get('scenario').split('_')[1]
+        write_episode_records(self.episodes(list(seeds)), self.output_path, name, self.agent,
+                              self.config.getfloat('control_interval_sec'))
+
+    def test_rewards(self, seeds):
+        """mean / std of the per-step global rewards of one greedy episode per seed, all episodes together."""
+        r = np.concatenate([reward[1:] for _, _, _, reward, _ in self.episodes(list(seeds))])
+        return np.mean(r), np.std(r)
+
+    def log_test(self, global_step, seeds, summary_writer=None):
+        """One test_reward.csv record (columns of train_reward.csv) and the TB scalar `test_reward`."""
+        mean, std = self.test_rewards(seeds)
+        self.data.append(dict(agent=self.agent, step=int(global_step), test_id=-1, avg_reward=mean, std_reward=std))
+        if summary_writer is not None:
+            summary_writer.add_scalar('test_reward', mean, int(global_step))
+        return mean
+
+    def write_csv(self, output_path):
+        import pandas as pd
+        pd.DataFrame(self.data).to_csv(output_path + 'test_reward.csv')
+
+
+def split_episodes(first, steps, action, reward, hs, vs, us):
+    """Host copies of one recorder pass -> (seed index, S, action [S, N], reward [S + 1], tr [S + 1, 3, N]) per
+    episode of S steps, in the layout CACCEnv keeps while it records (reward[0] = 0 and tr[0] is the reset state)."""
+    for b in range(len(steps)):
+        S = int(steps[b])
+        tr = np.empty((S + 1, 3, hs.shape[2]))
+        tr[:, 0], tr[:, 1], tr[:, 2] = hs[:S + 1, b], vs[:S + 1, b], us[:S + 1, b]
+        yield first + b, S, action[1:S + 1, b], np.ascontiguousarray(reward[:S + 1, b]), tr
+
+
+def write_episode_records(episodes, output_path, name, agent, dt):
+    """What Evaluator.run writes for these episodes: one `test %i, avg reward %.2f` log line each and, unless
+    output_path is None, <name>_<agent>_control.csv / _traffic.csv.  Episode k is numbered k + 1, as the one-env
+    env counts its resets from 0."""
+    control, traffic = [], []
+    for k, S, action, reward, tr in episodes:
+        if output_path is not None:
+            control.extend(control_record(k + 1, t, dt, action[t - 1], reward[t]) for t in range(1, S + 1))
+            traffic.append(traffic_frame(k + 1, tr, reward, dt))
+        logging.info('test %i, avg reward %.2f' % (k, np.mean(reward[1:].copy())))
+    if output_path is not None:
+        write_records(output_path, name, agent, control, traffic)

@@ -270,6 +270,21 @@ int nmarl_clip_rmsprop_step(const nmarl_model* m, float* params, float* grads, f
  *   scratch: device float [n_agent * ((s_dim + n_h) * 4*n_h + 4*n_h)]                                         */
 int nmarl_consensus_update(const nmarl_model* m, float* params, float* scratch, void* stream);
 
+/* ---- greedy evaluation episodes: episode recorder ----------------------------------------------
+ * Replaces the per-step recording of CACCEnv (_log_control_data / _log_traffic_data, envs/cacc_env.py:81-112,
+ * 225-241) for B envs that run one greedy episode each.  Call once with start = 1 right after the reset (records
+ * slot 0: the reset state, us = 0, reward 0; sets alive = 1, steps = 0), then with start = 0 after every env step.
+ * An env whose alive flag is set records the step at slot steps + 1, then clears alive if that step returned done
+ * (or reached slot T); envs that ended are not recorded again.  Reads the env's state in place; no host sync.
+ *   action int32 [N][B], greward double [B], done float [B] (the step's outputs; unused when start = 1)
+ *   hs, vs, us double [N][B] (env state after the step)     alive, steps int32 [B]
+ *   rec_action int32 [T+1][B][N] (slot 0 = 0)   rec_reward double [T+1][B]
+ *   rec_hs, rec_vs, rec_us double [T+1][B][N]                                                        */
+int nmarl_eval_record(int n_agent, int B, int T, int start, const int32_t* action, const double* greward,
+                      const float* done, const double* hs, const double* vs, const double* us,
+                      int32_t* alive, int32_t* steps, int32_t* rec_action, double* rec_reward,
+                      double* rec_hs, double* rec_vs, double* rec_us, void* stream);
+
 #pragma GCC visibility pop
 #ifdef __cplusplus
 }

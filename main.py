@@ -5,9 +5,11 @@ The reference's command line is kept verbatim (main.py:21-40 there) so existing 
     python main.py --base-dir D train    --config-dir F.ini
     python main.py --base-dir D evaluate [--evaluation-seeds s1,s2,...] [--demo]
 
-and so is the .ini surface (MODEL_CONFIG / TRAIN_CONFIG / ENV_CONFIG).  One optional new key: ENV_CONFIG.n_env
-(parallel episodes per process).  n_env = 1 runs the reference's one-episode-at-a-time Trainer; n_env > 1 the
-device-resident VecTrainer.  Agents: ia2c, ia2c_fp, ma2c_cu, ma2c_nc, ma2c_ic3, ma2c_dial on the CACC scenarios;
+and so is the .ini surface (MODEL_CONFIG / TRAIN_CONFIG / ENV_CONFIG).  Optional new keys: ENV_CONFIG.n_env
+(parallel episodes per process) and TRAIN_CONFIG.greedy_test (default false).  n_env = 1 runs the reference's
+one-episode-at-a-time Trainer; n_env > 1 the device-resident VecTrainer, which with greedy_test also logs the greedy
+test reward over ENV_CONFIG.test_seeds to data/test_reward.csv.  evaluate runs all seeds at once on the device and
+writes the files the reference's one-seed-at-a-time Evaluator writes.  Agents: ia2c, ia2c_fp, ma2c_cu, ma2c_nc, ma2c_ic3, ma2c_dial on the CACC scenarios;
 ATSC/SUMO environments are out of scope (SURVEY row 10).
 """
 import argparse
@@ -65,10 +67,12 @@ def init_agent(env, config, total_step, seed, **kw):
                              total_step, config, seed=seed, n_env=env.n_env, **kw)
 
 
-def _train_batched(env, model, total_step, log_interval, writer=None, output_path=None):
+def _train_batched(env, model, total_step, log_interval, writer=None, output_path=None, tester=None):
     """n_env > 1: whole updates on the device until total_step environment steps (summed over envs) are done.
     Every `log_interval` environment steps one record goes to data/train_reward.csv (and the TB scalar
-    `train_reward`): mean / std of the per-step global TRAINING reward of the last batch."""
+    `train_reward`): mean / std of the per-step global TRAINING reward of the last batch.  With a `tester`
+    (BatchedEvaluator, TRAIN_CONFIG.greedy_test) each record also runs one greedy episode per ENV_CONFIG test seed
+    with the current weights and adds a record to data/test_reward.csv (and the TB scalar `test_reward`)."""
     loop = U.VecTrainer(env, model)
     loop.start()
     done_steps, per_update = 0, model.n_step * env.n_env
@@ -79,8 +83,13 @@ def _train_batched(env, model, total_step, log_interval, writer=None, output_pat
         if loop.n_update % every == 0 or done_steps >= total_step:
             r = loop.log_rewards(done_steps, writer)
             logging.info('update %d, env steps %d, mean step reward %.2f' % (loop.n_update, done_steps, r))
+            if tester is not None:
+                r = tester.log_test(done_steps, env.test_seeds, writer)
+                logging.info('update %d, env steps %d, greedy test reward %.2f' % (loop.n_update, done_steps, r))
     if output_path is not None:
         loop.write_csv(output_path)
+        if tester is not None:
+            tester.write_csv(output_path)
     return done_steps
 
 
@@ -96,8 +105,10 @@ def train(args):
     if model is None:
         raise SystemExit(2)
     if env.n_env > 1:
+        greedy_test = cfg.getboolean('TRAIN_CONFIG', 'greedy_test', fallback=False)
+        tester = U.BatchedEvaluator(cfg['ENV_CONFIG'], model) if greedy_test else None
         final_step = _train_batched(env, model, steps['total_step'], steps['log_interval'],
-                                    U.make_summary_writer(dirs['log']), dirs['data'])
+                                    U.make_summary_writer(dirs['log']), dirs['data'], tester)
     else:
         counter = U.Counter(steps['total_step'], steps['test_interval'], steps['log_interval'])
         U.Trainer(env, model, counter, U.make_summary_writer(dirs['log']), output_path=dirs['data']).run()
@@ -119,8 +130,13 @@ def evaluate_fn(agent_dir, output_dir, seeds, port, demo):
     env = init_env(cfg['ENV_CONFIG'], port=port)
     env.init_test_seeds(seeds)
     model = init_agent(env, cfg['MODEL_CONFIG'], 0, 0)
-    if model is not None and model.load(agent_dir + '/model/'):
+    if model is None or not model.load(agent_dir + '/model/'):
+        return
+    if demo or not hasattr(model, 'engine'):
+        # --demo writes no files; agents without a device engine run the seeds one at a time
         U.Evaluator(env, model, output_dir, gui=demo).run()
+    else:
+        U.BatchedEvaluator(cfg['ENV_CONFIG'], model, output_dir).run(seeds)
 
 
 def evaluate(args):
