@@ -18,6 +18,13 @@ import torch
 
 from .. import _lib as L
 
+def tc_eligible(layout, n_env):
+    """True when a model of this layout with n_env envs runs the tensor-core kernels.  Same conditions as
+    nmarl_tc_fwd_supported / the bptt dispatch (csrc): whole 128-env tiles, encoders of at most one 32-deep k-block
+    and the width the tensor-core kernels are built for; everything else runs the FP32-FFMA kernels."""
+    return int(n_env) % 128 == 0 and layout.kx_pad <= 32 and layout.kp_pad <= 32 and layout.n_h == L.NH
+
+
 class PolicyEngine:
     def __init__(self, layout, n_env, n_step, hp, flat_params=None, device=None, rng_seed=0,
                  distance_mask=None, coop_gamma=-1.0, group=None, use_tc=None, shared_params=None):
@@ -51,10 +58,7 @@ class PolicyEngine:
         # tensor-core path: packed 3xTF32 operands; used by the kernels when B % 128 == 0
         if use_tc is None:
             use_tc = os.environ.get('NMARL_NO_TC', '0') != '1'
-        # same conditions as nmarl_tc_fwd_supported / the bptt dispatch (csrc): whole 128-env tiles, narrow encoders and
-        # the width the tensor-core kernels are built for; other widths run the FP32-FFMA kernels
-        self.use_tc = (bool(use_tc) and (self.B % 128 == 0) and layout.kx_pad <= 32 and layout.kp_pad <= 32
-                       and layout.n_h == L.NH)
+        self.use_tc = bool(use_tc) and tc_eligible(layout, self.B)
         self.wpack = torch.zeros(layout.n_wp, **f32) if self.use_tc else None
         self.tc_err = torch.zeros(1, dtype=torch.int32, device=dev)
         # tensor-core path: LSTM state (and its gradients) feature-major [N,64,B] so that lane == env accesses are

@@ -40,6 +40,18 @@ def _up4(x):
     return (int(x) + 3) // 4 * 4
 
 
+SMEM_LIMIT = 227 * 1024    # dynamic shared memory one CTA can opt in to on sm_90 (bytes)
+
+
+def ffma_fwd_smem_bytes(ld_in, s_dim, n_h):
+    """Dynamic shared memory of the FP32-FFMA cell kernel (csrc/cell_fwd.cu: fwd_smem_floats with BM = 64, KC = 16):
+    max(input tile, gate-weight ring, new-h tile) + [s | own h] tile + encoder-weight ring.  It is the only kernel
+    whose shared memory grows with the observation width (DESIGN 4.8)."""
+    bm, kc = 64, 16
+    region0 = max(bm * ld_in, 2 * kc * 4 * n_h, bm * (n_h + 4))
+    return 4 * (region0 + bm * (s_dim + n_h + 4) + 2 * kc * n_h)
+
+
 def ortho_init(shape, scale=np.sqrt(2)):
     """Orthogonal init from the GLOBAL NumPy stream (agents/utils.py:10-23): tall matrices get
     orthonormal columns, wide ones orthonormal rows, times sqrt(2)."""
@@ -207,6 +219,13 @@ class ModelLayout:
         self.kp_pad = _up4(n_a * max_nbr) if self.vid == L.NC else 0
         self.km_pad = {'ia2c': 0, 'ma2c_cu': 0, 'ma2c_ic3': NH}.get(v, NH * max_nbr)
         self.ld_in = self.kx_pad + self.kp_pad + self.km_pad
+        smem = ffma_fwd_smem_bytes(self.ld_in, self.s_dim, NH)
+        if smem > SMEM_LIMIT:
+            # every model can meet the FFMA kernel (B not a multiple of 128, greedy evaluation); nmarl_policy_step_*
+            # would refuse the launch with the same numbers
+            raise ValueError('observation encoder too wide: %d gathered inputs per agent (x %d + fingerprints %d + '
+                             'messages %d) need %d B of shared memory in the cell kernel, the limit is %d B'
+                             % (self.ld_in, self.kx_pad, self.kp_pad, self.km_pad, smem, SMEM_LIMIT))
         if self.concat:
             self.obs_stride = _up4(max(self.n_s_ls))
         else:

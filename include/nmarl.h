@@ -79,7 +79,9 @@ typedef struct {
                                          /*   width n_h = num_lstm: 16, 32 or 64 (NMARL_NH, the   */
                                          /*   only width with tensor-core kernels).  Every "64"   */
                                          /*   below is n_h, every "256" is 4 * n_h                */
-  int32_t obs_stride;                    /* floats per obs row                                  */
+  int32_t obs_stride;                    /* floats per obs row (>= x_w of every agent).  Only the  */
+                                         /*   first x_w columns of a row are ever read: what lies  */
+                                         /*   behind them is the caller's, and need not be zero    */
   int32_t kx_pad, kp_pad, km_pad;        /* padded (x4) widths of the x~ / p~ / m~ input segments */
   int32_t n_param, n_wt;                 /* flat buffer sizes (floats)                          */
   int32_t per_agent_norm;                /* 1: clip each agent's range separately (IA2C)        */
@@ -152,6 +154,14 @@ typedef struct {
   const double* uniforms;  /* [N][B] for NMARL_SAMPLE_UNIFORM                                  */
   const uint64_t* rng;     /* device [2] = {seed, counter} for NMARL_SAMPLE_PHILOX             */
   uint64_t rng_offset;     /* added to the device counter (distinct per call inside a graph)   */
+                           /* Keying, which any other binding has to match: Philox4x32-10 with  */
+                           /* key = (seed low, seed high) and counter words = (c low, c high,   */
+                           /* lane, 0x41435431), c = rng[1] + rng_offset (mod 2^64), lane =     */
+                           /* agent * B + env; u = ((w0 >> 5) * 2^26 + (w1 >> 6)) / 2^53 from   */
+                           /* output words 0, 1.  The call does not move rng[1]: a rollout      */
+                           /* passes offsets 0..T and then calls nmarl_rng_advance(rng, T + 1). */
+                           /* nmarl_cacc_reset draws from the same generator with counter =     */
+                           /* episode << 8 | platoon, lane = env and the tag 0x454e5601         */
   const int32_t* act_in;   /* v-call / train: [N][B] same-step actions                         */
   float* v;                /* v-call: [N][B]                                                   */
   const float* wpack;      /* packed 3xTF32 operands (nmarl_pack_weights) or NULL.  When set and  */

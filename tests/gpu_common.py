@@ -12,14 +12,33 @@ HP = dict(v_coef=0.5, e_coef=0.05, max_grad_norm=40.0, alpha=0.99, epsilon=1e-5,
           reward_norm=5000.0, reward_clip=-1.0)
 
 
-def make_pair(variant, B, T=4, seed=0, dtype=torch.float32, mask=None, n_a=4, hp=None, scale=0.3):
+def ladder_masks(cols=4):
+    """2 x cols ladder, row-major: the corner agents have 2 neighbours, the inner ones 3."""
+    r, c = np.divmod(np.arange(2 * cols), cols)
+    return ((np.abs(r[:, None] - r[None, :]) + np.abs(c[:, None] - c[None, :])) == 1).astype(int)
+
+
+def cut_chain_mask(n=8, cut=3):
+    """n-agent chain with agent `cut` cut off: it has no neighbours, and is nobody's neighbour."""
+    mask = chain_masks(n)[0]
+    mask[cut, :] = 0; mask[:, cut] = 0
+    return mask
+
+
+def widths(variant, mask, n_s, n_a):
+    """n_s_ls as the agents classes count it for an own-observation width n_s (gathered observations)."""
+    nm = [int(np.asarray(mask)[i].sum()) for i in range(len(mask))]
+    return {'ia2c': [n_s * (1 + k) for k in nm],
+            'ia2c_fp': [n_s * (1 + k) + n_a * k for k in nm]}.get(variant, [n_s] * len(mask))
+
+
+def make_pair(variant, B, T=4, seed=0, dtype=torch.float32, mask=None, n_a=4, hp=None, scale=0.3, n_s=5):
     from deeprl_network_b200.agents.engine import PolicyEngine
     from deeprl_network_b200.layout import ModelLayout
     if mask is None:
         mask, _ = chain_masks(8)
     N = len(mask)
-    nm = [int(mask[i].sum()) for i in range(N)]
-    n_s_ls = {'ia2c': [5 * (1 + k) for k in nm], 'ia2c_fp': [5 * (1 + k) + n_a * k for k in nm]}.get(variant, [5] * N)
+    n_s_ls = widths(variant, mask, n_s, n_a)
     lay = ModelLayout(variant, n_s_ls, n_a, mask, obs_mode='gather')
     params = random_params(lay.creation_order(), seed=seed, scale=scale)
     eng = PolicyEngine(lay, B, T, dict(HP if hp is None else hp), flat_params=lay.pack(params))
@@ -43,7 +62,10 @@ def check_apply_twice(eng, orc, lay, pad, lr=1e-2):
 
 
 def oracle_obs(lay, base):
-    """base [B, N, 5] own features -> per-agent oracle inputs (IA2C: own + neighbours concatenated)."""
+    """base [B, N, n_s] own features -> per-agent oracle inputs (IA2C: own + neighbours concatenated; pre-concatenated
+    observations of unequal width: the agent's first n_s_ls[i] columns)."""
+    if lay.concat:
+        return [base[:, i, :lay.n_s_ls[i]] for i in range(lay.N)]
     if lay.variant not in ('ia2c', 'ia2c_fp'):      # ia2c_fp: the fingerprints travel separately (ps)
         return [base[:, i] for i in range(lay.N)]
     return [np.concatenate([base[:, i]] + [base[:, j] for j in lay.nbr[i]], axis=1) for i in range(lay.N)]
@@ -63,10 +85,15 @@ def bn(t):
     return np.swapaxes(t.detach().cpu().numpy(), 0, 1)
 
 
-def obs_dev(lay, base):
-    B, N, _ = base.shape
-    o = np.zeros((N, B, lay.obs_stride), dtype=np.float32)
-    o[:, :, :5] = np.swapaxes(base, 0, 1)
+def obs_dev(lay, base, poison=False):
+    """base [B, N, w] -> device observation rows [N, B, obs_stride].  Agent i owns its first w columns (n_s_ls[i] of
+    them when the rows are pre-concatenated observations of unequal width); the columns behind them are padding, which
+    the kernels never read: zero, or NaN with `poison`."""
+    B, N, w = base.shape
+    o = np.full((N, B, lay.obs_stride), np.nan if poison else 0.0, dtype=np.float32)
+    for i in range(N):
+        wi = lay.n_s_ls[i] if lay.concat else w
+        o[i, :, :wi] = base[:, i, :wi]
     return to_dev(o)
 
 

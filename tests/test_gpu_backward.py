@@ -4,24 +4,26 @@ import numpy as np
 import pytest
 import torch
 
-from gpu_common import HP, bn, make_pair, nb, oracle_obs, to_dev
+from gpu_common import HP, bn, make_pair, nb, obs_dev, oracle_obs, to_dev
 
 pytestmark = pytest.mark.gpu
 VARIANTS = ['ma2c_nc', 'ma2c_ic3', 'ma2c_dial', 'ia2c', 'ia2c_fp', 'ma2c_cu']
 
 
-def _batch(eng, lay, T, B, seed=0, N=8):
+def _batch(eng, lay, T, B, seed=0, N=8, n_s=5, n_a=4, poison=False):
+    """Draw a training batch and load it into the engine's buffers.  poison: NaN in the padding columns of obs_buf."""
     rs = np.random.RandomState(seed)
-    base = rs.randn(T, B, N, 5).astype(np.float32)
-    fp = rs.dirichlet(np.ones(4), size=(T, B, N)).astype(np.float32)
-    acts = rs.randint(0, 4, size=(T, B, N))
+    base = rs.randn(T, B, N, n_s).astype(np.float32)
+    fp = rs.dirichlet(np.ones(n_a), size=(T, B, N)).astype(np.float32)
+    acts = rs.randint(0, n_a, size=(T, B, N))
     dones = np.zeros((T, B), dtype=np.float32); dones[0, ::2] = 1
     if T > 3:
         dones[3, 0] = 1
     Rs = rs.randn(T, B, N).astype(np.float32); Advs = rs.randn(T, B, N).astype(np.float32)
     c0 = (rs.randn(B, N, 64) * .5).astype(np.float32); h0 = (rs.rand(B, N, 64) - .5).astype(np.float32)
     eng.T_cur = T
-    eng.obs_buf[:T, :, :, :5].copy_(to_dev(np.transpose(base, (0, 2, 1, 3))))
+    for t in range(T):
+        eng.obs_buf[t].copy_(obs_dev(lay, base[t], poison=poison))
     eng.fp_buf[:T].copy_(to_dev(np.transpose(fp, (0, 2, 1, 3))))
     eng.act_buf[:T].copy_(to_dev(np.transpose(acts, (0, 2, 1)), torch.int32))
     eng.done_buf[:T].copy_(to_dev(dones))

@@ -14,10 +14,9 @@ import numpy as np
 import pytest
 import torch
 
-from gpu_common import HP, bn, check_apply_twice, nb, oracle_obs, to_dev
+from gpu_common import HP, bn, check_apply_twice, cut_chain_mask, nb, oracle_obs, to_dev, widths
 from helpers import random_params
 from oracle import nets
-from oracle.cacc import chain_masks
 
 pytestmark = pytest.mark.gpu
 N, CUT, N_A = 8, 3, 4
@@ -29,10 +28,8 @@ ISO_BIASES = {'ma2c_nc': ['nc/lstm_comm_%d/b_fp', 'nc/lstm_comm_%d/b_msg'], 'ma2
 def _pair(variant, B, T):
     from deeprl_network_b200.agents.engine import PolicyEngine
     from deeprl_network_b200.layout import ModelLayout
-    mask = chain_masks(N)[0]
-    mask[CUT, :] = 0; mask[:, CUT] = 0
-    nm = [int(mask[i].sum()) for i in range(N)]
-    n_s_ls = {'ia2c': [5 * (1 + k) for k in nm], 'ia2c_fp': [5 * (1 + k) + N_A * k for k in nm]}.get(variant, [5] * N)
+    mask = cut_chain_mask(N, CUT)
+    n_s_ls = widths(variant, mask, 5, N_A)
     lay = ModelLayout(variant, n_s_ls, N_A, mask, obs_mode='gather')
     assert lay.nbr[CUT] == [] and all(lay.nbr[i] for i in range(N) if i != CUT)
     params = random_params(lay.creation_order(), seed=6, scale=0.3)

@@ -13,10 +13,10 @@ VARIANTS = ['ma2c_nc', 'ma2c_ic3', 'ma2c_dial', 'ia2c', 'ia2c_fp', 'ma2c_cu']
 TOL = 1e-5
 
 
-def _inputs(B, N=8, seed=0):
+def _inputs(B, N=8, seed=0, n_s=5, n_a=4):
     rs = np.random.RandomState(seed)
-    base = rs.randn(B, N, 5).astype(np.float32)
-    fp = rs.dirichlet(np.ones(4), size=(B, N)).astype(np.float32)
+    base = rs.randn(B, N, n_s).astype(np.float32)
+    fp = rs.dirichlet(np.ones(n_a), size=(B, N)).astype(np.float32)
     done = (rs.rand(B) < 0.3).astype(np.float32)
     c0 = (rs.randn(B, N, 64) * 0.5).astype(np.float32)
     h0 = np.tanh(rs.randn(B, N, 64)).astype(np.float32) * 0.8

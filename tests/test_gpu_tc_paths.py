@@ -19,7 +19,7 @@ import pytest
 import torch
 from torch.overrides import TorchFunctionMode
 
-from gpu_common import HP, ScriptedEnv, nb, oracle_obs, to_dev
+from gpu_common import HP, ScriptedEnv, ladder_masks, nb, oracle_obs, to_dev, widths
 from helpers import golden, random_params
 from oracle import nets
 from oracle.cacc import chain_masks
@@ -66,9 +66,9 @@ CASES = []
 CUT = 3                         # topo 'chain8cut': the agent without neighbours
 
 
-def _case(cid, variant, B, T, purpose, topo='chain8', n_a=4, dones='mixed', kb=None):
-    CASES.append(pytest.param(dict(variant=variant, B=B, T=T, topo=topo, n_a=n_a, dones=dones, kb=kb, purpose=purpose),
-                              id=cid))
+def _case(cid, variant, B, T, purpose, topo='chain8', n_a=4, dones='mixed', kb=None, n_s=5):
+    CASES.append(pytest.param(dict(variant=variant, B=B, T=T, topo=topo, n_a=n_a, dones=dones, kb=kb, purpose=purpose,
+                              n_s=n_s), id=cid))
 
 
 for _v in VARIANTS:
@@ -94,6 +94,15 @@ _case('agents32-ma2c_nc', 'ma2c_nc', 128, 8, '32-agent chain (NMARL_MAX_AGENT): 
 for _na in (2, 7):
     for _v in ('ma2c_nc', 'ia2c'):
         _case('n_a%d-%s' % (_na, _v), _v, 128, 8, 'n_a != 4: the non-float4 head / dh branches', n_a=_na)
+# the edges of the shape envelope (tests/shape_cases.py) on every instantiation and on the fused rollout + BPTT path
+for _v in ('ma2c_nc', 'ma2c_ic3'):
+    _case('k30-' + _v, _v, 128, 8, 'n_s = 10, K = 30: the last k-step of the encoder k-block is partly padding', n_s=10)
+for _v in ('ma2c_nc', 'ia2c'):
+    _case('k32-ladder-' + _v, _v, 128, 8, '2x4 ladder, n_s = 8: K = 32 exactly for the inner agents, 24 for the corners',
+          topo='ladder8', n_s=8)
+_case('k32-ma2c_cu', 'ma2c_cu', 128, 8, 'n_s = 32: a single-source encoder that fills its k-block', n_s=32)
+_case('n_a3-ma2c_dial', 'ma2c_dial', 128, 8, 'n_a = 3: the generic heads beside the n_a == 4 fast path', n_a=3)
+_case('n_a1-ma2c_nc', 'ma2c_nc', 128, 8, 'n_a = 1: pi == 1, zero logit gradients', n_a=1)
 for _v in ('ma2c_nc', 'ia2c'):
     _case('wgrad-kb20-' + _v, _v, 128, 160, '20 k-blocks per split: one full segment, idle last split', kb=(20, [20]))
     _case('wgrad-kb21-' + _v, _v, 128, 168, '21 k-blocks per split: a 20-block segment then a 1-block segment',
@@ -178,14 +187,16 @@ def _model(c):
         n_s, n_a, mask = [int(x) for x in g['n_s_ls']], [int(x) for x in g['n_a_ls']], g['mask']
         lay = HeteroLayout(v, n_s, n_a, mask)
         return lay, (v, n_s, n_a, mask), n_s, n_a
-    mask = grid_masks(5)[0] if c['topo'] == 'grid5' else chain_masks(32 if c['topo'] == 'chain32' else 8)[0]
+    if c['topo'] == 'ladder8':
+        mask = ladder_masks(4)
+    else:
+        mask = grid_masks(5)[0] if c['topo'] == 'grid5' else chain_masks(32 if c['topo'] == 'chain32' else 8)[0]
     if c['topo'] == 'chain8cut':
         mask[CUT, :] = 0; mask[:, CUT] = 0
     N, n_a = len(mask), c['n_a']
-    nm = [int(mask[i].sum()) for i in range(N)]
-    n_s_ls = {'ia2c': [5 * (1 + k) for k in nm], 'ia2c_fp': [5 * (1 + k) + n_a * k for k in nm]}.get(v, [5] * N)
+    n_s_ls = widths(v, mask, c['n_s'], n_a)
     lay = ModelLayout(v, n_s_ls, n_a, mask, obs_mode='gather')
-    return lay, (v, n_s_ls, n_a, mask), [5] * N, [n_a] * N
+    return lay, (v, n_s_ls, n_a, mask), [c['n_s']] * N, [n_a] * N
 
 
 def _done_pattern(kind, rs, T, B):
