@@ -1,12 +1,12 @@
 // tc_wgrad.cu -- tensor-core (wgmma) weight gradients of every GEMM of the cell (gate matrix and the obs /
 // fingerprint / message encoders):   dW[ka][n] = sum over all (t, env) rows r of  A[r][ka] * D[r][n]
-// as 3xTF32 GEMMs with M = ka (each 128-lane job is two 64-lane CTAs), the contraction over rows split across CTAs
-// and a fixed-order reduce afterwards.
+// as 3xTF32 GEMMs with M = ka (one CTA per 128-lane job tile: two MMA warpgroups of 64 lanes each share every
+// streamed D^T tile), the contraction over rows split across CTAs and a fixed-order reduce afterwards.
 //   A operand: the saved activations are feature-major ([t][agent][feature][env]); operand row = feature ka, so
-//              a thread reads 8 consecutive envs (32 contiguous bytes), splits hi/lo and stores them into the
-//              swizzled shared-memory ring.
+//              a thread reads the 32 consecutive envs of one k-block (one 128-byte line), splits hi/lo and stores
+//              them into the swizzled shared-memory ring.
 //   B operand: D^T, K-major over rows, was written by the backward cell kernel as ready-made [hi | lo]
-//              128B-swizzled tiles (dz: 256 rows, encoder pre-activation grads: 192/128/64 rows); the producer
+//              128B-swizzled tiles (dz: 256 rows, encoder pre-activation grads: 192/128/64 rows); one thread
 //              bulk-copies the needed row range of the tile per 32 env rows.
 //   Biases:    the obs-encoder job carries an extra all-ones lane and spans every column of the dpre tile, which
 //              yields all encoder bias gradients for free; the gate bias is a coalesced column sum of dz.
@@ -19,15 +19,38 @@ namespace {
 using namespace tcrow;
 
 enum { J_GATE0 = 0, J_GATE1, J_ENC_X, J_ENC_M0, J_ENC_M1, J_COUNT };
-// Row threads: 4 sets x 64 feature lanes; set s produces envs [8s, 8s + 8) of every 32-env k-block.
-constexpr int WG_LANES = 64, WG_SETS = 4, WA = 32 / WG_SETS;
-constexpr int WG_A_THREADS = WG_LANES * WG_SETS;
-constexpr int WG_MMA_WARP0 = WG_A_THREADS / 32, WG_THREADS = WG_A_THREADS + 128;
-constexpr int WG_STAGES = 3;
-constexpr size_t WG_SMEM = 1024 + (size_t)WG_STAGES * STAGE_BYTES + A_SLOTS * A_SLOT_BYTES + 16 * 8;
+// Warpgroup 0: the A producers, one thread per feature lane of the 128-lane tile.  Warpgroups 1 and 2: the MMA
+// warpgroups of lanes 0-63 and 64-127.
+constexpr int WG_LANES = 128, WG_HALF = 64;
+constexpr int WG_A_THREADS = WG_LANES, WG_THREADS = WG_A_THREADS + 2 * 128;
+// A slot: [hi | lo] 128-row x 32-deep swizzled tiles; rows 64-127 of each form a second 1024-aligned 8 KB tile
+constexpr uint32_t WG_A_TILE = WG_LANES * 128, WG_A_SLOT = 2 * WG_A_TILE;
+// The B stages ([hi | lo] N-row tiles, 256 N bytes) and the A slots share one 224 KB ring; the depths depend on the
+// job's N (wg_depths), so the narrow jobs run a much deeper ring than the gate jobs.
+constexpr uint32_t WG_RING = 224 * 1024;
+constexpr int WG_MAX_BARS = 32;
+constexpr size_t WG_SMEM = 1024 + WG_RING + WG_MAX_BARS * 8;
 static_assert(WG_SMEM <= 232448, "wgrad rings exceed the 227 KB of dynamic shared memory");
-static_assert(WG_LANES == ROWS, "A tiles of the wgrad kernel have the cell kernels' 64 rows");
+static_assert(WG_HALF == ROWS, "each MMA warpgroup covers the 64 rows of one wgmma");
+// Register split (setmaxnreg): the CTA is launched with 168 registers per thread (384 x 168 = 64 512); the producer
+// warpgroup drops to 120 and each MMA warpgroup (128 accumulators) rises to 192: 128 x 120 + 256 x 192 = 64 512.
+constexpr int WG_REGS_A = 120, WG_REGS_MMA = 192;
+static_assert(WG_A_THREADS * WG_REGS_A + 256 * WG_REGS_MMA <= WG_THREADS * 168, "setmaxnreg split exceeds the CTA's registers");
 constexpr int SEG_KB = 20;       // k-blocks (of 32 rows) accumulated in registers before the accumulator is drained
+
+// B stages and A slots per job width: N = 256: 2 x 64 KB + 3 x 32 KB; N = 192: 3 x 48 KB + 2 x 32 KB;
+// N = 128: 4 x 32 KB + 3 x 32 KB; N = 64: 6 x 16 KB + 4 x 32 KB (DESIGN 4.1)
+__device__ __forceinline__ void wg_depths(int N, int& S, int& A) {
+  S = N >= 256 ? 2 : (N >= 192 ? 3 : (N >= 128 ? 4 : 6));
+  A = (int)((WG_RING - (uint32_t)S * 256u * (uint32_t)N) / WG_A_SLOT);
+  if (A > 4) A = 4;
+}
+
+// position in a ring of `n` entries: index and the parity of its current use
+struct RingPos {
+  int idx = 0; uint32_t ph = 0;
+  __device__ __forceinline__ void next(int n) { if (++idx == n) { idx = 0; ph ^= 1u; } }
+};
 
 struct TcWgK {
   int B, T, splits, ndp;
@@ -37,6 +60,7 @@ struct TcWgK {
   long long ws_off[J_COUNT];     // float offset of each job's partial block [splits][N_agents][128][N_job]
   int jobs[J_COUNT]; int n_jobs; // job kinds present
   int* err;
+  long long* prof;               // debug: per-k-block clock64 stamps of CTA (split 0, agent 0) of every job, or NULL
 };
 
 struct JobDesc {
@@ -70,20 +94,34 @@ __device__ __forceinline__ JobDesc job_desc(const nmarl_model& m, const TcWgK& k
 // RAW: the D^T tiles hold raw fp32 once.  One tile per k-block is copied into the hi half of the stage; the A-producer
 // threads split it in place into the same rounded [hi | lo] pair the packed tiles carry (tc::split_tf32) and signal
 // b_split, so the split overlaps the previous k-block's MMAs instead of preceding the k-block's own.
+//
+// Hand-offs per k-block q (B stage st = q mod S, A slot = q mod A; every wait is on an mbarrier):
+//   thread 0 of MMA warpgroup 0 bulk-copies tile q into st once b_empty[st] reports that every active warpgroup has
+//   retired k-block q - S;  the producers fill the A slot once a_empty reports the same for q - A, then (RAW) split
+//   stage st once b_full[st] has landed;  each active MMA warpgroup waits for b_split / b_full and a_full, issues its
+//   12 wgmma against its own 64 A rows and the shared B stage, retires them and arrives on a_empty and b_empty (one
+//   arrival per warp, so both count 4 x the active warpgroups).
+// A warpgroup whose 64 lanes all lie beyond the job's real lanes (ka_cnt + ones lane + fingerprints) issues nothing:
+// the reduce never reads those lanes.
 template <bool RAW>
 __global__ void __launch_bounds__(WG_THREADS, 1) tc_wgrad_kernel(const __grid_constant__ nmarl_model m,
                                                                  const __grid_constant__ TcWgK k) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* bst = smem;
-  uint8_t* ast = smem + (size_t)WG_STAGES * STAGE_BYTES;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(ast + A_SLOTS * A_SLOT_BYTES);
-  uint64_t* b_full = bars, *a_full = bars + WG_STAGES, *a_empty = a_full + A_SLOTS, *b_split = a_empty + A_SLOTS;
-  static_assert(2 * WG_STAGES + 2 * A_SLOTS <= 16, "mbarrier area of WG_SMEM");
 
-  const int sp = blockIdx.x, jslot = blockIdx.y >> 1, mh = blockIdx.y & 1, i = blockIdx.z;
+  const int sp = blockIdx.x, jslot = blockIdx.y, i = blockIdx.z;
   const int kind = k.jobs[jslot];
   const JobDesc d = job_desc(m, k, kind, i);
+  const int lanes = d.ka_cnt > 0 ? d.ka_cnt + d.ones + d.p_cnt : 0;  // lanes the reduce reads (all zero if no features)
+  const int nact = (lanes + WG_HALF - 1) / WG_HALF;                   // active MMA warpgroups: 0, 1 or 2
+  if (nact == 0) return;                                              // nothing is read from this CTA's block
+  int S, AS;
+  wg_depths(d.N, S, AS);
+  uint8_t* bst = smem;
+  uint8_t* ast = smem + (size_t)S * 256 * d.N;
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + WG_RING);
+  uint64_t *b_full = bars, *b_split = b_full + S, *b_empty = b_split + S, *a_full = b_empty + S, *a_empty = a_full + AS;
+
   const int N_agents = m.n_agent;
   const int tid = threadIdx.x, warp = tid >> 5;
   const int bpt = k.B / 32;                                           // 32-row k-blocks per time step
@@ -94,29 +132,22 @@ __global__ void __launch_bounds__(WG_THREADS, 1) tc_wgrad_kernel(const __grid_co
   float* wsj = k.ws + k.ws_off[jslot] + ((size_t)sp * N_agents + i) * 128 * d.N;
 
   if (tid == 0) {
-    for (int s = 0; s < WG_STAGES; ++s) tc::mbar_init(&b_full[s], 1);
-    for (int s = 0; s < A_SLOTS; ++s) { tc::mbar_init(&a_full[s], WG_A_THREADS); tc::mbar_init(&a_empty[s], 128); }
-    for (int s = 0; s < WG_STAGES; ++s) tc::mbar_init(&b_split[s], WG_A_THREADS);
+    for (int s = 0; s < S; ++s) { tc::mbar_init(&b_full[s], 1); tc::mbar_init(&b_split[s], WG_A_THREADS); tc::mbar_init(&b_empty[s], 4 * nact); }
+    for (int s = 0; s < AS; ++s) { tc::mbar_init(&a_full[s], WG_A_THREADS); tc::mbar_init(&a_empty[s], 4 * nact); }
     tc::fence_barrier_init();
   }
   __syncthreads();
   const uint32_t tile_bytes = (uint32_t)d.N * 128u;                   // hi (or lo) part staged per k-block
-  // byte offset of the D^T tile of (t, 32-env block rb): [hi | lo] pairs, or single raw tiles packed inside each
-  // time step's (unchanged) [hi | lo]-sized slab
-  auto bt_tile = [&](int t, int rb) -> const uint8_t* {
-    const size_t pair = (size_t)(2 * d.tile_rows * 128);
-    const size_t off = RAW ? (size_t)t * N_agents * bpt * pair + ((size_t)i * bpt + rb) * (pair / 2)
-                           : (((size_t)t * N_agents + i) * bpt + rb) * pair;
-    return reinterpret_cast<const uint8_t*>(d.BT) + off;
-  };
 
-  if (warp < WG_MMA_WARP0) {
-    // ---- A producers: feature lane `row` of this CTA, envs [set * WA, set * WA + WA) of every k-block ----------------
-    const int row = tid % WG_LANES, set = tid / WG_LANES;
-    const int ka = mh * WG_LANES + row;                               // feature within the job's 128-lane tile
+  if (warp < WG_A_THREADS / 32) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(WG_REGS_A));
+    // ---- A producers: feature lane `row` of the job's 128-lane tile, all 32 envs of every k-block ----------------
+    const int row = tid;
+    const bool on = row < WG_HALF * nact;                             // an active warpgroup reads this row
+    const int ka = row;
     const bool one = d.ones && ka == d.ka_cnt;
     const bool is_p = ka > d.ka_cnt && ka <= d.ka_cnt + d.p_cnt;
-    const bool real = ka < d.ka_cnt || is_p;
+    const bool real = on && (ka < d.ka_cnt || is_p);
     const int feat = is_p ? d.p_feat0 + (ka - d.ka_cnt - 1) : d.a_feat0 + ka;
     // Feature-major state path: the forward kernel does not save h^ (= (1 - done) * own h_seq[t]) and, for NeurComm,
     // m~ (= the neighbours' h_seq[t]) a second time; those operand rows are read from the state sequence itself.
@@ -129,53 +160,61 @@ __global__ void __launch_bounds__(WG_THREADS, 1) tc_wgrad_kernel(const __grid_co
         hs_agent = m.agent[i].nbr[fm / NH]; hs_unit = fm % NH;
       }
     }
-    // the A operand of k-block q: 8 consecutive envs of this thread's feature (global loads; issued two k-blocks AHEAD
-    // so that their latency hides behind the barrier waits of the current k-block)
-    auto load_x = [&](int q, float (&x)[WA]) {
+    // the A operand of k-block q: the 32 envs of this thread's feature (global loads; issued two k-blocks AHEAD so
+    // that their latency hides behind the barrier waits of the current k-block)
+    auto load_x = [&](int q, float (&x)[32]) {
       const int kb = kb0 + q, t = kb / bpt, rb = kb - t * bpt;
       if (hs_agent >= 0) {
-        const float* src = k.h_seq + (((size_t)t * N_agents + hs_agent) * NH + hs_unit) * k.B + rb * 32 + set * WA;
+        const float* src = k.h_seq + (((size_t)t * N_agents + hs_agent) * NH + hs_unit) * k.B + rb * 32;
 #pragma unroll
-        for (int p = 0; p < WA / 4; ++p) {
+        for (int p = 0; p < 8; ++p) {
           const float4 v = __ldg(reinterpret_cast<const float4*>(src + 4 * p));
           x[4 * p] = v.x; x[4 * p + 1] = v.y; x[4 * p + 2] = v.z; x[4 * p + 3] = v.w;
         }
         if (hs_mask) {
-          const float* dn = k.done_pre + (size_t)t * k.B + rb * 32 + set * WA;
+          const float* dn = k.done_pre + (size_t)t * k.B + rb * 32;
 #pragma unroll
-          for (int p = 0; p < WA / 4; ++p) {
+          for (int p = 0; p < 8; ++p) {
             const float4 v = __ldg(reinterpret_cast<const float4*>(dn + 4 * p));
             x[4 * p] *= 1.0f - v.x; x[4 * p + 1] *= 1.0f - v.y; x[4 * p + 2] *= 1.0f - v.z; x[4 * p + 3] *= 1.0f - v.w;
           }
         }
       } else if (real) {
-        const float* src = d.A + (((size_t)t * N_agents + i) * d.F_A + feat) * k.B + rb * 32 + set * WA;
+        const float* src = d.A + (((size_t)t * N_agents + i) * d.F_A + feat) * k.B + rb * 32;
 #pragma unroll
-        for (int p = 0; p < WA / 4; ++p) {
+        for (int p = 0; p < 8; ++p) {
           const float4 v = __ldcs(reinterpret_cast<const float4*>(src + 4 * p));
           x[4 * p] = v.x; x[4 * p + 1] = v.y; x[4 * p + 2] = v.z; x[4 * p + 3] = v.w;
         }
       } else {
 #pragma unroll
-        for (int j = 0; j < WA; ++j) x[j] = one ? 1.0f : 0.0f;
+        for (int j = 0; j < 32; ++j) x[j] = one ? 1.0f : 0.0f;
       }
     };
-    float xa[WA], xb[WA];                     // the operands of the next two k-blocks (two loads in flight per thread)
-    auto emit_a = [&](int q, float (&x)[WA]) {
-      const int slot = q & (A_SLOTS - 1);
-      tc::mbar_wait(&a_empty[slot], ((q / A_SLOTS) & 1) ^ 1, k.err, 11);
-      uint8_t* hi = ast + slot * A_SLOT_BYTES;
-      tc::st_hilo8(hi, hi + A_TILE, (uint32_t)row, (uint32_t)(set * WA), x);
-      tc::fence_proxy_async();
-      tc::mbar_arrive(&a_full[slot]);
+    float xa[32], xb[32];                     // the operands of the next two k-blocks (two loads in flight per thread)
+    RingPos as, bs;
+    auto emit_a = [&](int q, float (&x)[32]) {
+      tc::mbar_wait(&a_empty[as.idx], as.ph ^ 1, k.err, 11);
+      if (on) {
+        uint8_t* hi = ast + (size_t)as.idx * WG_A_SLOT;
+#pragma unroll
+        for (int c = 0; c < 4; ++c) {
+          float x8[8];
+#pragma unroll
+          for (int j = 0; j < 8; ++j) x8[j] = x[8 * c + j];
+          tc::st_hilo8(hi, hi + WG_A_TILE, (uint32_t)row, (uint32_t)(8 * c), x8);
+        }
+        tc::fence_proxy_async();
+      }
+      tc::mbar_arrive(&a_full[as.idx]);
+      as.next(AS);
       if (q + 2 < nkb) load_x(q + 2, x);        // refill this buffer; it is consumed two k-blocks from now
       if constexpr (RAW) {
         // split the raw D^T tile of this k-block into its [hi | lo] pair once it has landed.  In order: the stage is
-        // refilled with k-block q + WG_STAGES only after the MMAs of q, which wait for this split, have retired.
-        const int st = q % WG_STAGES;
-        tc::mbar_wait(&b_full[st], (q / WG_STAGES) & 1, k.err, 31);
-        float4* bhi = reinterpret_cast<float4*>(bst + (size_t)st * STAGE_BYTES);
-        float4* blo = reinterpret_cast<float4*>(bst + (size_t)st * STAGE_BYTES + tile_bytes);
+        // refilled with k-block q + S only after the MMAs of q, which wait for this split, have retired.
+        tc::mbar_wait(&b_full[bs.idx], bs.ph, k.err, 31);
+        float4* bhi = reinterpret_cast<float4*>(bst + (size_t)bs.idx * 2 * tile_bytes);
+        float4* blo = reinterpret_cast<float4*>(bst + (size_t)bs.idx * 2 * tile_bytes + tile_bytes);
         for (uint32_t e = (uint32_t)tid; e < tile_bytes / 16; e += WG_A_THREADS) {
           const float4 v = bhi[e];
           float4 h, lo4;
@@ -185,7 +224,8 @@ __global__ void __launch_bounds__(WG_THREADS, 1) tc_wgrad_kernel(const __grid_co
           blo[e] = lo4;
         }
         tc::fence_proxy_async();
-        tc::mbar_arrive(&b_split[st]);
+        tc::mbar_arrive(&b_split[bs.idx]);
+        bs.next(S);
       }
     };
     if (nkb > 0) load_x(0, xa);
@@ -195,24 +235,35 @@ __global__ void __launch_bounds__(WG_THREADS, 1) tc_wgrad_kernel(const __grid_co
       if (q + 1 < nkb) emit_a(q + 1, xb);
     }
   } else {
-    // ---- MMA warpgroup; its thread 0 also bulk-copies the D^T tiles into the WG_STAGES ring --------------------------
+    // ---- MMA warpgroup g (lanes 64 g .. 64 g + 63); thread 0 of warpgroup 0 also bulk-copies the D^T tiles ----------
     // Segmented accumulation: the accumulator is drained into the CTA's workspace slot every SEG_KB k-blocks
     // (240 MMAs) and the segment sums are added up there with ordinary round-to-nearest fp32 adds, which bounds the
     // error growth of a single long accumulation chain.
-    const int t = tid - WG_MMA_WARP0 * 32, w = t >> 5, l = t & 31;
+    const int g = warp / 4 - 1;
+    if (g >= nact) return;                    // lanes beyond the job's real ones: no MMAs, no drain
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(WG_REGS_MMA));
+    const int t = tid - (g + 1) * 128, w = t >> 5, l = t & 31;
+    const bool issuer = g == 0 && t == 0;
     // workspace block layout [column n][lane ka]
-    float* out = wsj + mh * WG_LANES + 16 * w + (l >> 2);
-    auto fetch = [&](int q) {
-      const int kb = kb0 + q, st = q % WG_STAGES;
+    float* out = wsj + g * WG_HALF + 16 * w + (l >> 2);
+    long long* prof = (issuer && k.prof != nullptr && sp == 0 && i == 0) ? k.prof + (size_t)jslot * 1024 : nullptr;
+    if (prof) { prof[0] = clock64(); prof[3] = kind | (d.N << 8); }
+    auto fetch = [&](int q, int st) {
+      const int kb = kb0 + q;
       const int tt = kb / bpt, rb = kb - tt * bpt;
-      const uint8_t* tile = bt_tile(tt, rb);
+      // byte offset of the D^T tile of (t, 32-env block rb): [hi | lo] pairs, or single raw tiles packed inside each
+      // time step's (unchanged) [hi | lo]-sized slab
+      const size_t pair = (size_t)(2 * d.tile_rows * 128);
+      const size_t off = RAW ? (size_t)tt * N_agents * bpt * pair + ((size_t)i * bpt + rb) * (pair / 2)
+                             : (((size_t)tt * N_agents + i) * bpt + rb) * pair;
+      const uint8_t* tile = reinterpret_cast<const uint8_t*>(d.BT) + off;
+      uint8_t* dst = bst + (size_t)st * 2 * tile_bytes;
       tc::mbar_arrive_expect_tx(&b_full[st], RAW ? tile_bytes : 2 * tile_bytes);
-      tc::bulk_g2s(bst + (size_t)st * STAGE_BYTES, tile + (size_t)d.n_row0 * 128, tile_bytes, &b_full[st]);
-      if (!RAW)
-        tc::bulk_g2s(bst + (size_t)st * STAGE_BYTES + tile_bytes, tile + (size_t)(d.tile_rows + d.n_row0) * 128, tile_bytes, &b_full[st]);
+      tc::bulk_g2s(dst, tile + (size_t)d.n_row0 * 128, tile_bytes, &b_full[st]);
+      if (!RAW) tc::bulk_g2s(dst + tile_bytes, tile + (size_t)(d.tile_rows + d.n_row0) * 128, tile_bytes, &b_full[st]);
     };
-    if (t == 0)
-      for (int q = 0; q < WG_STAGES && q < nkb; ++q) fetch(q);
+    if (issuer)
+      for (int q = 0; q < S && q < nkb; ++q) fetch(q, q);
     float acc[128];
 #pragma unroll
     for (int j = 0; j < 128; ++j) acc[j] = 0.f;
@@ -229,25 +280,32 @@ __global__ void __launch_bounds__(WG_THREADS, 1) tc_wgrad_kernel(const __grid_co
         }
       }
     };
+    RingPos as, bs;
     for (int q = 0; q < nkb; ++q) {
-      const int st = q % WG_STAGES, slot = q & (A_SLOTS - 1);
       const bool seg_first = (q % SEG_KB) == 0;
-      uint8_t* b = bst + (size_t)st * STAGE_BYTES;
-      if constexpr (RAW) tc::mbar_wait(&b_split[st], (q / WG_STAGES) & 1, k.err, 33);   // landed and split (A producers)
-      else tc::mbar_wait(&b_full[st], (q / WG_STAGES) & 1, k.err, 31);
-      tc::mbar_wait(&a_full[slot], (q / A_SLOTS) & 1, k.err, 32);
-      uint8_t* a = ast + slot * A_SLOT_BYTES;
+      uint8_t* b = bst + (size_t)bs.idx * 2 * tile_bytes;
+      if constexpr (RAW) tc::mbar_wait(&b_split[bs.idx], bs.ph, k.err, 33);   // landed and split (A producers)
+      else tc::mbar_wait(&b_full[bs.idx], bs.ph, k.err, 31);
+      if (prof && q < 300) prof[4 + 3 * q] = clock64();
+      tc::mbar_wait(&a_full[as.idx], as.ph, k.err, 32);
+      if (prof && q < 300) prof[5 + 3 * q] = clock64();
+      uint8_t* a = ast + (size_t)as.idx * WG_A_SLOT + g * (WG_A_TILE / 2);
       tc::wgmma_fence();
-      tc::wgmma_kblock_3x(d.N, acc, tc::smem_desc_sw128(a), tc::smem_desc_sw128(a + A_TILE), tc::smem_desc_sw128(b),
+      tc::wgmma_kblock_3x(d.N, acc, tc::smem_desc_sw128(a), tc::smem_desc_sw128(a + WG_A_TILE), tc::smem_desc_sw128(b),
                           tc::smem_desc_sw128(b + tile_bytes), 4, seg_first);
       tc::wgmma_commit();
       tc::wgmma_wait_all();
-      tc::mbar_arrive(&a_empty[slot]);
-      mma_wg_sync();                              // every thread has retired the k-block: stage st is free
-      if (t == 0 && q + WG_STAGES < nkb) fetch(q + WG_STAGES);
+      if (prof && q < 300) prof[6 + 3 * q] = clock64();
+      if (l == 0) { tc::mbar_arrive(&a_empty[as.idx]); tc::mbar_arrive(&b_empty[bs.idx]); }
+      if (issuer && q + S < nkb) {
+        tc::mbar_wait(&b_empty[bs.idx], bs.ph, k.err, 34);         // every active warpgroup has retired k-block q
+        fetch(q + S, bs.idx);
+      }
+      as.next(AS); bs.next(S);
       if ((q + 1) % SEG_KB == 0 || q + 1 == nkb) drain(q >= SEG_KB);
     }
-    if (nkb == 0) drain(false);                // acc is zero: the reduce reads every lane of the block
+    if (nkb == 0) drain(false);                // acc is zero: the reduce reads every real lane of the block
+    if (prof) { prof[1] = min(nkb, 300); prof[2] = clock64(); }
   }
 }
 
@@ -323,7 +381,7 @@ int job_N(const nmarl_model* m, int kind) {
 int nmarl_tc_ndp(const nmarl_model* m) { return m->variant == NMARL_NC ? 192 : (m->variant == NMARL_IA2C ? 64 : 128); }
 
 int nmarl_tc_wgrad_splits(int n_agent) {
-  int s = 33;                                   // 2 gate tiles x 2 halves x 33 x 8 agents = 1056 CTAs = 8 waves of 132 SMs
+  int s = 33;                                   // 4 jobs x 33 x 8 agents = 1056 CTAs = 8 waves of 132 SMs
   while (4 * s * n_agent > 132 * 8 && s > 1) s = (s + 1) / 2;
   return s;
 }
@@ -342,7 +400,7 @@ int nmarl_tc_launch_wgrads(const nmarl_model* m, int B, int T, const float* sv_s
   TcWgK k{};
   k.B = B; k.T = T; k.splits = nmarl_tc_wgrad_splits(m->n_agent); k.ndp = nmarl_tc_ndp(m);
   k.sv_sh = sv_sh; k.sv_xin = sv_xin; k.dzT = dzT; k.dpT = dpT; k.ws = ws; k.err = err;
-  k.h_seq = h_seq; k.done_pre = done_pre;
+  k.h_seq = h_seq; k.done_pre = done_pre; k.prof = g_nmarl_prof;
   k.n_jobs = job_list(m, k.jobs);
   long long off = 0;
   for (int j = 0; j < k.n_jobs; ++j) { k.ws_off[j] = off; off += (long long)k.splits * m->n_agent * 128 * job_N(m, k.jobs[j]); }
@@ -356,7 +414,7 @@ int nmarl_tc_launch_wgrads(const nmarl_model* m, int B, int T, const float* sv_s
   gate_bias_reduce_kernel<<<dim3(NG / 32, m->n_agent), 256, 0, st_bias>>>(*m, sv_dz, B / 32, T, grads);
   NMARL_LAUNCH_CHECK();
   if (ev_wgrad) NMARL_CUDA(cudaEventRecord((cudaEvent_t)ev_wgrad[0], st));
-  const dim3 grid(k.splits, 2 * k.n_jobs, m->n_agent);               // y: (job, 64-lane half of its 128-lane tile)
+  const dim3 grid(k.splits, k.n_jobs, m->n_agent);                   // one CTA per (row split, 128-lane job tile, agent)
   if (raw_tiles) tc_wgrad_kernel<true><<<grid, WG_THREADS, WG_SMEM, st>>>(*m, k);
   else tc_wgrad_kernel<false><<<grid, WG_THREADS, WG_SMEM, st>>>(*m, k);
   NMARL_LAUNCH_CHECK();
