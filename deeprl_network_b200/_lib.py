@@ -9,8 +9,14 @@ import os
 
 import torch
 
-MAX_AGENT, MAX_NBR, NH, MAX_NA = 128, 4, 64, 8       # NH: the width of the tensor-core kernels
+MAX_AGENT, MAX_NBR, NH, MAX_NA = 128, 4, 64, 16      # NH: the width of the tensor-core kernels; n_a < MAX_NA
 WIDTHS = (16, 32, 64)                                  # LSTM widths (num_lstm) the FFMA kernels run
+
+
+def head_width(n_a):
+    """Floats per sv_dlv row (nmarl_head_width): the n_a logits plus the value slot, rounded up to 8 or 16."""
+    return 8 if n_a < 8 else 16
+
 IA2C, NC, IC3, DIAL = 0, 1, 2, 3
 SAMPLE_NONE, SAMPLE_UNIFORM, SAMPLE_PHILOX, SAMPLE_GREEDY = 0, 1, 2, 3
 CATCHUP, SLOWDOWN = 0, 1

@@ -349,7 +349,7 @@ class PolicyEngine:
         self.sv_sh = z(T, N, B, lay.s_dim + NH)
         self.sv_gates = z(T, N, B, 4 * NH)
         self.sv_enc = z(T, N, B, 2 * NH) if self.variant in ('ma2c_ic3', 'ma2c_dial') else None
-        self.sv_dlv = z(T, N, B, 8)
+        self.sv_dlv = z(T, N, B, L.head_width(self.n_a))      # d(loss)/d(logits), then d(loss)/d(v) at column n_a
         # tensor-core path: sv_dz holds per-tile gate-bias partial sums, sv_dpre is unused (operand tiles instead)
         self.sv_dz = z(T, N, B // 32, 4 * NH) if self.use_tc else z(T, N, B, 4 * NH)
         self.sv_dpre = z(4) if self.use_tc else z(T, N, B, 3 * NH)

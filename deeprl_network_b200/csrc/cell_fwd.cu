@@ -28,7 +28,7 @@ __host__ __device__ inline size_t fwd_smem_floats(const nmarl_model& m) {
   return fwd_region0_floats<BM, KC, H>(m) + (size_t)BM * (m.s_dim + H + 4) + (size_t)2 * KC * H;
 }
 
-template <int VAR, int MODE, int BM, int TY, int H>
+template <int VAR, int MODE, int BM, int TY, int H, int HW>
 __global__ void __launch_bounds__(H / 4 * TY) cell_fwd_kernel(const __grid_constant__ nmarl_model m,
                                                           const __grid_constant__ FwdK k) {
   constexpr int NT = H / 4 * TY, TM = BM / TY, KC = 16;
@@ -261,7 +261,7 @@ __global__ void __launch_bounds__(H / 4 * TY) cell_fwd_kernel(const __grid_const
       const float4 t4 = *reinterpret_cast<const float4*>(Hs + r * LDH + 4 * u4);
       h[4 * u4] = t4.x; h[4 * u4 + 1] = t4.y; h[4 * u4 + 2] = t4.z; h[4 * u4 + 3] = t4.w;
     }
-    float pi[NMARL_MAX_NA];
+    float pi[HW];
     if (MODE != MODE_V) {
       float mx = -3.0e38f;
       for (int c = 0; c < n_a; ++c) {
@@ -287,7 +287,7 @@ __global__ void __launch_bounds__(H / 4 * TY) cell_fwd_kernel(const __grid_const
         double u;
         if (a.sample_mode == NMARL_SAMPLE_UNIFORM) u = a.uniforms[row];
         else u = philox_u01(a.rng[0], a.rng[1] + a.rng_offset, (uint32_t)row, 0x41435431u);
-        double cdf[NMARL_MAX_NA];
+        double cdf[HW];
         double s = 0.0;
         for (int c = 0; c < n_a; ++c) { s += (double)pi[c]; cdf[c] = s; }
         for (int c = 0; c < n_a; ++c) act += ((cdf[c] / s) <= u) ? 1 : 0;
@@ -307,7 +307,7 @@ __global__ void __launch_bounds__(H / 4 * TY) cell_fwd_kernel(const __grid_const
       const int act = a.act_in[row];
       const float R = k.Rs[row], Adv = k.Advs[row];
       const float cs = k.loss_scale;
-      float lp[NMARL_MAX_NA], g[NMARL_MAX_NA];
+      float lp[HW], g[HW];
       float ent = 0.f, dot = 0.f;
       for (int c = 0; c < n_a; ++c) {
         const float pc = fminf(fmaxf(pi[c], 1e-10f), 1.0f);
@@ -318,8 +318,8 @@ __global__ void __launch_bounds__(H / 4 * TY) cell_fwd_kernel(const __grid_const
         if (c == act) g[c] += -cs * Adv * in_rng / pc;
       }
       for (int c = 0; c < n_a; ++c) dot += pi[c] * g[c];
-      float* dl = k.sv_dlv + row * 8;
-      for (int c = 0; c < 8; ++c) dl[c] = (c < n_a) ? pi[c] * (g[c] - dot) : 0.f;
+      float* dl = k.sv_dlv + row * HW;
+      for (int c = 0; c < HW; ++c) dl[c] = (c < n_a) ? pi[c] * (g[c] - dot) : 0.f;
       dl[n_a] = -k.v_coef * cs * (R - v);
       l_pol = -lp[act] * Adv;
       l_val = (R - v) * (R - v);
@@ -400,10 +400,10 @@ constexpr int FWD_BM = 64;
 NMARL_PARAMS_FIT(nmarl_model, FwdK);                                             // cell_fwd_kernel
 NMARL_PARAMS_FIT(nmarl_model, int, const float*, const float*, float*);          // dial_msg_kernel
 
-template <int VAR, int MODE, int H>
+template <int VAR, int MODE, int H, int HW>
 int launch_fwd(const nmarl_model* m, const FwdK& k, cudaStream_t st) {
   constexpr int TY = nmarl_ffma_ty(H);
-  auto kern = cell_fwd_kernel<VAR, MODE, FWD_BM, TY, H>;
+  auto kern = cell_fwd_kernel<VAR, MODE, FWD_BM, TY, H, HW>;
   const size_t smem = fwd_smem_floats<FWD_BM, 16, H>(*m) * sizeof(float);
   NMARL_CHECK(smem <= 227 * 1024, "policy_step: shared memory %zu B exceeds 227 KB", smem);
   static size_t configured = 0;     // per instantiation
@@ -417,25 +417,30 @@ int launch_fwd(const nmarl_model* m, const FwdK& k, cudaStream_t st) {
   return 0;
 }
 
-template <int VAR, int MODE>
+template <int VAR, int MODE, int HW>
 int launch_fwd_width(const nmarl_model* m, const FwdK& k, cudaStream_t st) {
   switch (nmarl_n_h(*m)) {
-    case 16: return launch_fwd<VAR, MODE, 16>(m, k, st);
-    case 32: return launch_fwd<VAR, MODE, 32>(m, k, st);
-    case 64: return launch_fwd<VAR, MODE, 64>(m, k, st);
+    case 16: return launch_fwd<VAR, MODE, 16, HW>(m, k, st);
+    case 32: return launch_fwd<VAR, MODE, 32, HW>(m, k, st);
+    case 64: return launch_fwd<VAR, MODE, 64, HW>(m, k, st);
   }
   nmarl_set_error("n_h %d has no FFMA kernel", nmarl_n_h(*m));
   return 1;
+}
+
+template <int VAR, int MODE>
+int launch_fwd_head(const nmarl_model* m, const FwdK& k, cudaStream_t st) {
+  return nmarl_head_width(m->n_a) == 8 ? launch_fwd_width<VAR, MODE, 8>(m, k, st) : launch_fwd_width<VAR, MODE, 16>(m, k, st);
 }
 
 template <int MODE>
 int dispatch_fwd(const nmarl_model* m, const FwdK& k, cudaStream_t st) {
   if (nmarl_tc_fwd_supported(m, &k.a)) return nmarl_tc_launch_fwd(m, k, MODE, st);
   switch (m->variant) {
-    case NMARL_IA2C: return launch_fwd_width<NMARL_IA2C, MODE>(m, k, st);
-    case NMARL_NC: return launch_fwd_width<NMARL_NC, MODE>(m, k, st);
-    case NMARL_IC3: return launch_fwd_width<NMARL_IC3, MODE>(m, k, st);
-    case NMARL_DIAL: return launch_fwd_width<NMARL_DIAL, MODE>(m, k, st);
+    case NMARL_IA2C: return launch_fwd_head<NMARL_IA2C, MODE>(m, k, st);
+    case NMARL_NC: return launch_fwd_head<NMARL_NC, MODE>(m, k, st);
+    case NMARL_IC3: return launch_fwd_head<NMARL_IC3, MODE>(m, k, st);
+    case NMARL_DIAL: return launch_fwd_head<NMARL_DIAL, MODE>(m, k, st);
   }
   nmarl_set_error("unknown variant %d", m->variant);
   return 1;

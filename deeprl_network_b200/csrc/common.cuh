@@ -15,6 +15,10 @@ __host__ __device__ constexpr bool nmarl_width_ok(int h) { return h == 16 || h =
 // n_h from the descriptor: s_dim = 3 * n_h for NeurComm ([s_x | s_p | s_m]), n_h for every other cell
 __host__ __device__ inline int nmarl_n_h(const nmarl_model& m) { return m.variant == NMARL_NC ? m.s_dim / 3 : m.s_dim; }
 constexpr int nmarl_ffma_ty(int h) { return 1024 / h; }
+// Head width HW: the n_a logits plus the value slot, rounded up to 8 (n_a <= 7) or 16 (n_a 8..15).  It is the row
+// width of sv_dlv and the size of the per-row head arrays; every kernel that touches the heads takes it as a template
+// parameter and the host dispatches on nmarl_head_width(m->n_a).
+__host__ __device__ constexpr int nmarl_head_width(int n_a) { return n_a < 8 ? 8 : 16; }
 __host__ __device__ constexpr int nmarl_log2(int x) { return x <= 1 ? 0 : 1 + nmarl_log2(x / 2); }
 
 void nmarl_set_error(const char* fmt, ...);

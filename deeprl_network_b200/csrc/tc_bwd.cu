@@ -13,7 +13,7 @@ using namespace tcrow;
 // RAW (the default; nmarl_bwd_args.raw_tiles): the operand tiles for the weight-gradient GEMMs are stored once as raw
 // fp32 instead of as a [hi | lo] pair; the weight-gradient kernel splits them in shared memory with the same
 // tc::split_tf32, so both forms feed its MMAs identical operands.
-template <int VAR, bool FM, bool RAW>
+template <int VAR, bool FM, bool RAW, int HW>
 __global__ void __launch_bounds__(TC_THREADS, 1) tc_cell_bwd_kernel(const __grid_constant__ nmarl_model m,
                                                                     const __grid_constant__ BwdK k) {
   extern __shared__ uint8_t smem_raw[];
@@ -62,12 +62,15 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_cell_bwd_kernel(const __grid
     // ---- total dh and dc for the thread's units --------------------------------------------------------------
     float dh[EW], dct[EW], dzo[EW];
     {
-      const float4 d0 = *reinterpret_cast<const float4*>(k.sv_dlv + row * 8);
-      const float4 d1 = *reinterpret_cast<const float4*>(k.sv_dlv + row * 8 + 4);
-      const float dl[8] = {d0.x, d0.y, d0.z, d0.w, d1.x, d1.y, d1.z, d1.w};
+      float dl[HW];                           // sv_dlv row: HW floats, d(logits) then d(v) at column n_a
+#pragma unroll
+      for (int q = 0; q < HW / 4; ++q) {
+        const float4 d4 = *reinterpret_cast<const float4*>(k.sv_dlv + row * HW + 4 * q);
+        dl[4 * q] = d4.x; dl[4 * q + 1] = d4.y; dl[4 * q + 2] = d4.z; dl[4 * q + 3] = d4.w;
+      }
       float dv = 0.f;
 #pragma unroll
-      for (int cc = 0; cc < 8; ++cc) if (cc == n_a) dv = dl[cc];
+      for (int cc = 0; cc < HW; ++cc) if (cc == n_a) dv = dl[cc];
       float4 vw[EW / 4];
 #pragma unroll
       for (int q4 = 0; q4 < EW / 4; ++q4) vw[q4] = __ldg(reinterpret_cast<const float4*>(P + ag.o_v_w + e0) + q4);
@@ -79,7 +82,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_cell_bwd_kernel(const __grid
           s = fmaf(dl[0], w4.x, s); s = fmaf(dl[1], w4.y, s); s = fmaf(dl[2], w4.z, s); s = fmaf(dl[3], w4.w, s);
         } else {
 #pragma unroll
-          for (int cc = 0; cc < NMARL_MAX_NA - 1; ++cc)
+          for (int cc = 0; cc < HW - 1; ++cc)
             if (cc < n_a) s = fmaf(dl[cc], __ldg(P + ag.o_pi_w + (e0 + j) * n_a + cc), s);
         }
         dh[j] = fmaf(dv, f4get(vw[j >> 2], j & 3), s);
@@ -264,9 +267,9 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_cell_bwd_kernel(const __grid
 
 NMARL_PARAMS_FIT(nmarl_model, BwdK);                                             // tc_cell_bwd_kernel
 
-template <int VAR, bool FM, bool RAW>
+template <int VAR, bool FM, bool RAW, int HW>
 int launch_tc_bwd_fm(const nmarl_model* m, const BwdK& k, cudaStream_t st) {
-  auto kern = tc_cell_bwd_kernel<VAR, FM, RAW>;
+  auto kern = tc_cell_bwd_kernel<VAR, FM, RAW, HW>;
   static bool configured = false;
   if (!configured) {
     NMARL_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TC_SMEM));
@@ -278,10 +281,15 @@ int launch_tc_bwd_fm(const nmarl_model* m, const BwdK& k, cudaStream_t st) {
   return 0;
 }
 
+template <int VAR, int HW>
+int launch_tc_bwd_hw(const nmarl_model* m, const BwdK& k, cudaStream_t st) {
+  if (k.raw_tiles) return k.state_fm ? launch_tc_bwd_fm<VAR, true, true, HW>(m, k, st) : launch_tc_bwd_fm<VAR, false, true, HW>(m, k, st);
+  return k.state_fm ? launch_tc_bwd_fm<VAR, true, false, HW>(m, k, st) : launch_tc_bwd_fm<VAR, false, false, HW>(m, k, st);
+}
+
 template <int VAR>
 int launch_tc_bwd(const nmarl_model* m, const BwdK& k, cudaStream_t st) {
-  if (k.raw_tiles) return k.state_fm ? launch_tc_bwd_fm<VAR, true, true>(m, k, st) : launch_tc_bwd_fm<VAR, false, true>(m, k, st);
-  return k.state_fm ? launch_tc_bwd_fm<VAR, true, false>(m, k, st) : launch_tc_bwd_fm<VAR, false, false>(m, k, st);
+  return nmarl_head_width(m->n_a) == 8 ? launch_tc_bwd_hw<VAR, 8>(m, k, st) : launch_tc_bwd_hw<VAR, 16>(m, k, st);
 }
 
 }  // namespace

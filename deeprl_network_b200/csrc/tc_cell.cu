@@ -26,11 +26,12 @@ namespace {
 
 using namespace tcrow;
 
-template <int VAR, int MODE, bool FM>
+template <int VAR, int MODE, bool FM, int HW>
 __global__ void __launch_bounds__(TC_THREADS, 1) tc_cell_fwd_kernel(const __grid_constant__ nmarl_model m,
                                                                     const __grid_constant__ FwdK k) {
   constexpr bool SAVE = (MODE == MODE_TRAIN || MODE == MODE_PS);   // store activations for BPTT
   constexpr bool SAMPLE = (MODE == MODE_P || MODE == MODE_PS);     // p-call: sample actions
+  static_assert(HW <= EW, "a set's HW partial head sums live in its EW gate-f staging columns");
   extern __shared__ uint8_t smem_raw[];
   const Smem sm = smem_map(smem_raw);
   KbEnt* sched = sm.sched;
@@ -260,9 +261,9 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_cell_fwd_kernel(const __grid
     // ---- LSTM cell update for hidden units [e0, e0 + EW), 8 at a time; partial head sums -----------------------
     tc::mbar_wait(sm.acc_full, 0, a.tc_err, 13);
     STAMP();
-    float logit[NMARL_MAX_NA];
+    float logit[HW];
 #pragma unroll
-    for (int cc = 0; cc < NMARL_MAX_NA; ++cc) logit[cc] = 0.f;
+    for (int cc = 0; cc < HW; ++cc) logit[cc] = 0.f;
     float v = 0.f;
 #pragma unroll 1
     for (int u0 = e0; u0 < e0 + EW; u0 += 8) {
@@ -326,7 +327,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_cell_fwd_kernel(const __grid
 #pragma unroll
           for (int x = 0; x < 8; ++x)
 #pragma unroll
-            for (int cc = 0; cc < NMARL_MAX_NA; ++cc)
+            for (int cc = 0; cc < HW; ++cc)
               if (cc < n_a) logit[cc] = fmaf(hn[x], __ldg(P + ag.o_pi_w + (u0 + x) * n_a + cc), logit[cc]);
         }
       }
@@ -344,13 +345,13 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_cell_fwd_kernel(const __grid
     if (VAR == NMARL_DIAL && MODE != MODE_V) produce_act(c, s0);
 
     // ---- heads: combine the NSET partial sums of a row in fixed order, then softmax / sampling / loss -------
-    // The partial sums of set s go to staging columns [NH + s*EW, +8) of the row: gate-f cells that only this
-    // thread has read, and that the DIAL message GEMM (columns [0, NH)) does not overwrite.
+    // The partial sums of set s go to staging columns [NH + s*EW, +HW) of the row (HW - 1 logits, then v): gate-f
+    // cells that only this thread has read, and that the DIAL message GEMM (columns [0, NH)) does not overwrite.
     {
       float* hp = sm.acc;
 #pragma unroll
-      for (int cc = 0; cc < NMARL_MAX_NA - 1; ++cc) hp[acc_idx(r, NH + e0 + cc)] = logit[cc];
-      hp[acc_idx(r, NH + e0 + NMARL_MAX_NA - 1)] = v;
+      for (int cc = 0; cc < HW - 1; ++cc) hp[acc_idx(r, NH + e0 + cc)] = logit[cc];
+      hp[acc_idx(r, NH + e0 + HW - 1)] = v;
     }
     STAMP();
     row_barrier();
@@ -358,27 +359,27 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_cell_fwd_kernel(const __grid
     float l_pol = 0.f, l_val = 0.f, l_ent = 0.f;
     if (set == 0) {
 #pragma unroll
-      for (int cc = 0; cc < NMARL_MAX_NA; ++cc) logit[cc] = 0.f;
+      for (int cc = 0; cc < HW; ++cc) logit[cc] = 0.f;
       v = 0.f;
 #pragma unroll
       for (int s = 0; s < NSET; ++s) {
         const float* hp = sm.acc;
 #pragma unroll
-        for (int cc = 0; cc < NMARL_MAX_NA - 1; ++cc) logit[cc] += hp[acc_idx(r, NH + s * EW + cc)];
-        v += hp[acc_idx(r, NH + s * EW + NMARL_MAX_NA - 1)];
+        for (int cc = 0; cc < HW - 1; ++cc) logit[cc] += hp[acc_idx(r, NH + s * EW + cc)];
+        v += hp[acc_idx(r, NH + s * EW + HW - 1)];
       }
-      float pi[NMARL_MAX_NA];
+      float pi[HW];
       if (MODE != MODE_V) {
         float mx = -3.0e38f;
 #pragma unroll
-        for (int cc = 0; cc < NMARL_MAX_NA; ++cc)
+        for (int cc = 0; cc < HW; ++cc)
           if (cc < n_a) { logit[cc] += __ldg(P + ag.o_pi_b + cc); mx = fmaxf(mx, logit[cc]); }
         float se = 0.f;
 #pragma unroll
-        for (int cc = 0; cc < NMARL_MAX_NA; ++cc)
+        for (int cc = 0; cc < HW; ++cc)
           if (cc < n_a) { pi[cc] = expf(logit[cc] - mx); se += pi[cc]; } else pi[cc] = 0.f;
 #pragma unroll
-        for (int cc = 0; cc < NMARL_MAX_NA; ++cc)
+        for (int cc = 0; cc < HW; ++cc)
           if (cc < n_a) { pi[cc] = pi[cc] / se; if (a.pi != nullptr) a.pi[row * n_a + cc] = pi[cc]; }
       }
       if (SAMPLE && a.action != nullptr && a.sample_mode != NMARL_SAMPLE_NONE) {
@@ -386,25 +387,25 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_cell_fwd_kernel(const __grid
         if (a.sample_mode == NMARL_SAMPLE_GREEDY) {
           float best = pi[0];
 #pragma unroll
-          for (int cc = 1; cc < NMARL_MAX_NA; ++cc) if (cc < n_a && pi[cc] > best) { best = pi[cc]; act = cc; }
+          for (int cc = 1; cc < HW; ++cc) if (cc < n_a && pi[cc] > best) { best = pi[cc]; act = cc; }
         } else {
           double u;
           if (a.sample_mode == NMARL_SAMPLE_UNIFORM) u = a.uniforms[row];
           else u = philox_u01(a.rng[0], a.rng[1] + a.rng_offset, (uint32_t)row, 0x41435431u);
-          double cdf[NMARL_MAX_NA];
+          double cdf[HW];
           double s = 0.0;
 #pragma unroll
-          for (int cc = 0; cc < NMARL_MAX_NA; ++cc) { if (cc < n_a) s += (double)pi[cc]; cdf[cc] = s; }
+          for (int cc = 0; cc < HW; ++cc) { if (cc < n_a) s += (double)pi[cc]; cdf[cc] = s; }
           if (a.sample_mode == NMARL_SAMPLE_UNIFORM) {
             // host-supplied uniforms: np.random.choice's rule verbatim (cdf /= cdf[-1]; searchsorted(cdf, u, 'right'))
 #pragma unroll
-            for (int cc = 0; cc < NMARL_MAX_NA; ++cc) if (cc < n_a) act += ((cdf[cc] / s) <= u) ? 1 : 0;
+            for (int cc = 0; cc < HW; ++cc) if (cc < n_a) act += ((cdf[cc] / s) <= u) ? 1 : 0;
           } else {
             // device Philox stream (no NumPy stream to reproduce): the same inverse-cdf draw without the four fp64
             // divisions -- they are the longest dependent chain of the kernel's tail
             const double us = u * s;
 #pragma unroll
-            for (int cc = 0; cc < NMARL_MAX_NA; ++cc) if (cc < n_a) act += (cdf[cc] <= us) ? 1 : 0;
+            for (int cc = 0; cc < HW; ++cc) if (cc < n_a) act += (cdf[cc] <= us) ? 1 : 0;
           }
           act = min(act, n_a - 1);
         }
@@ -419,10 +420,10 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_cell_fwd_kernel(const __grid
         const int act = a.act_in[row];
         const float R = k.Rs[row], Adv = k.Advs[row];
         const float cs = k.loss_scale;
-        float g[NMARL_MAX_NA];
+        float g[HW];
         float ent = 0.f, dot = 0.f, lpa = 0.f;
 #pragma unroll
-        for (int cc = 0; cc < NMARL_MAX_NA; ++cc) {
+        for (int cc = 0; cc < HW; ++cc) {
           g[cc] = 0.f;
           if (cc < n_a) {
             const float pc = fminf(fmaxf(pi[cc], 1e-10f), 1.0f);
@@ -434,14 +435,15 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_cell_fwd_kernel(const __grid
             dot += pi[cc] * g[cc];
           }
         }
-        float dl[8];
+        float dl[HW];
 #pragma unroll
-        for (int cc = 0; cc < 8; ++cc) dl[cc] = (cc < n_a) ? pi[cc] * (g[cc] - dot) : 0.f;
+        for (int cc = 0; cc < HW; ++cc) dl[cc] = (cc < n_a) ? pi[cc] * (g[cc] - dot) : 0.f;
         const float dvv = -k.v_coef * cs * (R - v);
 #pragma unroll
-        for (int cc = 0; cc < 8; ++cc) if (cc == n_a) dl[cc] = dvv;
-        *reinterpret_cast<float4*>(k.sv_dlv + row * 8) = make_float4(dl[0], dl[1], dl[2], dl[3]);
-        *reinterpret_cast<float4*>(k.sv_dlv + row * 8 + 4) = make_float4(dl[4], dl[5], dl[6], dl[7]);
+        for (int cc = 0; cc < HW; ++cc) if (cc == n_a) dl[cc] = dvv;
+#pragma unroll
+        for (int q = 0; q < HW / 4; ++q)
+          *reinterpret_cast<float4*>(k.sv_dlv + row * HW + 4 * q) = make_float4(dl[4 * q], dl[4 * q + 1], dl[4 * q + 2], dl[4 * q + 3]);
         l_pol = -lpa * Adv; l_val = (R - v) * (R - v); l_ent = ent;
       }
     }
@@ -477,9 +479,9 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_cell_fwd_kernel(const __grid
 
 NMARL_PARAMS_FIT(nmarl_model, FwdK);                                             // tc_cell_fwd_kernel
 
-template <int VAR, int MODE, bool FM>
+template <int VAR, int MODE, bool FM, int HW>
 int launch_tc_fm(const nmarl_model* m, const FwdK& k, cudaStream_t st) {
-  auto kern = tc_cell_fwd_kernel<VAR, MODE, FM>;
+  auto kern = tc_cell_fwd_kernel<VAR, MODE, FM, HW>;
   static bool configured = false;
   if (!configured) {
     NMARL_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TC_SMEM));
@@ -493,9 +495,14 @@ int launch_tc_fm(const nmarl_model* m, const FwdK& k, cudaStream_t st) {
   return 0;
 }
 
+template <int VAR, int MODE, int HW>
+int launch_tc_hw(const nmarl_model* m, const FwdK& k, cudaStream_t st) {
+  return k.a.state_fm ? launch_tc_fm<VAR, MODE, true, HW>(m, k, st) : launch_tc_fm<VAR, MODE, false, HW>(m, k, st);
+}
+
 template <int VAR, int MODE>
 int launch_tc(const nmarl_model* m, const FwdK& k, cudaStream_t st) {
-  return k.a.state_fm ? launch_tc_fm<VAR, MODE, true>(m, k, st) : launch_tc_fm<VAR, MODE, false>(m, k, st);
+  return nmarl_head_width(m->n_a) == 8 ? launch_tc_hw<VAR, MODE, 8>(m, k, st) : launch_tc_hw<VAR, MODE, 16>(m, k, st);
 }
 
 template <int VAR>

@@ -101,7 +101,7 @@ __global__ void __launch_bounds__(256) transpose_all_kernel(const __grid_constan
 }
 
 // ============================ K9: one reverse step of the cell ==================================
-template <int VAR, int BM, int TY, int H>
+template <int VAR, int BM, int TY, int H, int HW>
 __global__ void __launch_bounds__(H / 4 * TY) cell_bwd_kernel(const __grid_constant__ nmarl_model m,
                                                           const __grid_constant__ BwdK k) {
   constexpr int TM = BM / TY, KC = 16;
@@ -119,13 +119,13 @@ __global__ void __launch_bounds__(H / 4 * TY) cell_bwd_kernel(const __grid_const
   const float* __restrict__ P = k.params;
 
   // ---- phase 0/1: total dh, gate derivatives ---------------------------------------------------
-  float wpi[4][NMARL_MAX_NA];               // W_pi rows of this thread's 4 units, then W_v
+  float wpi[4][HW];                         // W_pi rows of this thread's 4 units, then W_v
 #pragma unroll
   for (int j = 0; j < 4; ++j) {
 #pragma unroll
-    for (int c = 0; c < NMARL_MAX_NA; ++c) wpi[j][c] = 0.f;
+    for (int c = 0; c < HW; ++c) wpi[j][c] = 0.f;
     for (int c = 0; c < n_a; ++c) wpi[j][c] = __ldg(P + ag.o_pi_w + (4 * tx + j) * n_a + c);
-    wpi[j][NMARL_MAX_NA - 1] = __ldg(P + ag.o_v_w + 4 * tx + j);
+    wpi[j][HW - 1] = __ldg(P + ag.o_v_w + 4 * tx + j);
   }
 #pragma unroll
   for (int q = 0; q < TM; ++q) {
@@ -136,17 +136,27 @@ __global__ void __launch_bounds__(H / 4 * TY) cell_bwd_kernel(const __grid_const
     if (r < rows) {
       const int b = b0 + r;
       const size_t row = (size_t)i * B + b;
-      const float4 d0 = *reinterpret_cast<const float4*>(k.sv_dlv + row * 8);
-      const float4 d1 = *reinterpret_cast<const float4*>(k.sv_dlv + row * 8 + 4);
-      const float dl[8] = {d0.x, d0.y, d0.z, d0.w, d1.x, d1.y, d1.z, d1.w};
-      const float dv = dl[n_a];
       float dh[4], dc[4] = {0.f, 0.f, 0.f, 0.f};
+      auto head_dh = [&](const float (&dl)[HW]) {  // sv_dlv row: HW floats, d(logits) then d(v) at column n_a
+        const float dv = dl[n_a];
 #pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        float s = 0.f;
+        for (int j = 0; j < 4; ++j) {
+          float s = 0.f;
 #pragma unroll
-        for (int c = 0; c < NMARL_MAX_NA - 1; ++c) s = fmaf(c < n_a ? dl[c] : 0.f, wpi[j][c], s);
-        dh[j] = fmaf(dv, wpi[j][NMARL_MAX_NA - 1], s);
+          for (int c = 0; c < HW - 1; ++c) s = fmaf(c < n_a ? dl[c] : 0.f, wpi[j][c], s);
+          dh[j] = fmaf(dv, wpi[j][HW - 1], s);
+        }
+      };
+      const float4 d0 = *reinterpret_cast<const float4*>(k.sv_dlv + row * HW);
+      const float4 d1 = *reinterpret_cast<const float4*>(k.sv_dlv + row * HW + 4);
+      if constexpr (HW == 8) {
+        const float dl[8] = {d0.x, d0.y, d0.z, d0.w, d1.x, d1.y, d1.z, d1.w};
+        head_dh(dl);
+      } else {
+        const float4 d2 = *reinterpret_cast<const float4*>(k.sv_dlv + row * HW + 8);
+        const float4 d3 = *reinterpret_cast<const float4*>(k.sv_dlv + row * HW + 12);
+        const float dl[16] = {d0.x, d0.y, d0.z, d0.w, d1.x, d1.y, d1.z, d1.w, d2.x, d2.y, d2.z, d2.w, d3.x, d3.y, d3.z, d3.w};
+        head_dh(dl);
       }
       if (k.has_next) {
         const float4 r4 = *reinterpret_cast<const float4*>(k.dh_in + row * H + 4 * tx);
@@ -505,18 +515,19 @@ __global__ void wgrad_reduce_kernel(const __grid_constant__ WgRedK k) {
 struct HeadK {
   int N, B, T, splits, n_a, fm;
   const float* h1;           // h_seq + N*B*n_h  (h_t, t = 0..T-1)
-  const float* dlv;          // [T][N][B][8]
+  const float* dlv;          // [T][N][B][HW]
   const int32_t* act;        // [T][N][B]
-  float* ws;                 // [splits][N][HEAD_WS]
+  float* ws;                 // [splits][N][head_ws(HW)]
 };
-constexpr int HEAD_WS = 64 * 8 + 8 + NMARL_MAX_NBR * NMARL_MAX_NA;   // per (split, agent): n_h x 8, then the extras
+// per (split, agent): n_h x HW products, then the extras: HW column sums of dlv and HW one-hot sums per neighbour slot
+__host__ __device__ constexpr int head_ws(int hw) { return 64 * hw + hw + NMARL_MAX_NBR * hw; }
 
-template <int H>
+template <int H, int HW>
 __global__ void __launch_bounds__(256) head_wgrad_kernel(const __grid_constant__ nmarl_model m,
                                                         const __grid_constant__ HeadK k) {
   // red[part][unit][c]: 256 / H row parts of H units (only H = 64 runs feature-major)
   constexpr int NPARTS = 256 / H;
-  __shared__ float red[NPARTS][H][9];
+  __shared__ float red[NPARTS][H][HW + 1];
   __shared__ float red2[256];
   const int sp = blockIdx.x, i = blockIdx.y;
   const nmarl_agent& ag = m.agent[i];
@@ -527,128 +538,166 @@ __global__ void __launch_bounds__(256) head_wgrad_kernel(const __grid_constant__
     if constexpr (H == 64) {       // feature-major state exists on the tensor-core path only (n_h = 64)
       // feature-major h ([t][agent][unit][env]): the coalesced direction is env, so a warp covers 32 consecutive envs and
       // 8 of the 64 units; 8 x 8 accumulators per thread, one shuffle tree over the envs at the end.  (Reading it with
-      // lanes = units touched 32 different 128-byte lines per load: 0.94 ms for 0.5 GB.)
+      // lanes = units touched 32 different 128-byte lines per load: 0.94 ms for 0.5 GB.)  HW = 16 takes the rows twice,
+      // 8 dlv columns per pass: 8 x 16 accumulators would be 128 live floats per thread.
       const long nb32 = R / 32, per32 = (nb32 + k.splits - 1) / k.splits;
       const long blk_begin = (long)sp * per32, blk_end = min(nb32, blk_begin + per32);
       r_begin = blk_begin * 32; r_end = blk_end * 32;
       const int lane = tid & 31, w = tid >> 5;
-      float a[8][8];
 #pragma unroll
-      for (int uu = 0; uu < 8; ++uu)
+      for (int c0 = 0; c0 < HW; c0 += 8) {
+        float a[8][8];
 #pragma unroll
-        for (int c = 0; c < 8; ++c) a[uu][c] = 0.f;
-      for (long blk = blk_begin; blk < blk_end; ++blk) {
-        const long r = blk * 32 + lane, t = r / k.B, b = r - t * k.B;
-        const size_t row = ((size_t)t * k.N + i) * k.B + b;
-        const float4 d0 = *reinterpret_cast<const float4*>(k.dlv + row * 8);
-        const float4 d1 = *reinterpret_cast<const float4*>(k.dlv + row * 8 + 4);
-        const float dl[8] = {d0.x, d0.y, d0.z, d0.w, d1.x, d1.y, d1.z, d1.w};
-        const float* hp = k.h1 + (((size_t)t * k.N + i) * NH + 8 * w) * k.B + b;
+        for (int uu = 0; uu < 8; ++uu)
 #pragma unroll
-        for (int uu = 0; uu < 8; ++uu) {
-          const float hv = hp[(size_t)uu * k.B];
+          for (int c = 0; c < 8; ++c) a[uu][c] = 0.f;
+        for (long blk = blk_begin; blk < blk_end; ++blk) {
+          const long r = blk * 32 + lane, t = r / k.B, b = r - t * k.B;
+          const size_t row = ((size_t)t * k.N + i) * k.B + b;
+          const float4 d0 = *reinterpret_cast<const float4*>(k.dlv + row * HW + c0);
+          const float4 d1 = *reinterpret_cast<const float4*>(k.dlv + row * HW + c0 + 4);
+          const float dl[8] = {d0.x, d0.y, d0.z, d0.w, d1.x, d1.y, d1.z, d1.w};
+          const float* hp = k.h1 + (((size_t)t * k.N + i) * NH + 8 * w) * k.B + b;
 #pragma unroll
-          for (int c = 0; c < 8; ++c) a[uu][c] = fmaf(hv, dl[c], a[uu][c]);
+          for (int uu = 0; uu < 8; ++uu) {
+            const float hv = hp[(size_t)uu * k.B];
+#pragma unroll
+            for (int c = 0; c < 8; ++c) a[uu][c] = fmaf(hv, dl[c], a[uu][c]);
+          }
         }
+#pragma unroll
+        for (int uu = 0; uu < 8; ++uu)
+#pragma unroll
+          for (int c = 0; c < 8; ++c) {
+            float x = a[uu][c];
+            for (int o = 16; o > 0; o >>= 1) x += __shfl_xor_sync(0xffffffffu, x, o);
+            if (lane == 0) {
+              red[0][8 * w + uu][c0 + c] = x; red[1][8 * w + uu][c0 + c] = 0.f;
+              red[2][8 * w + uu][c0 + c] = 0.f; red[3][8 * w + uu][c0 + c] = 0.f;
+            }
+          }
       }
-#pragma unroll
-      for (int uu = 0; uu < 8; ++uu)
-#pragma unroll
-        for (int c = 0; c < 8; ++c) {
-          float x = a[uu][c];
-          for (int o = 16; o > 0; o >>= 1) x += __shfl_xor_sync(0xffffffffu, x, o);
-          if (lane == 0) { red[0][8 * w + uu][c] = x; red[1][8 * w + uu][c] = 0.f; red[2][8 * w + uu][c] = 0.f; red[3][8 * w + uu][c] = 0.f; }
-        }
     }
   } else {
   const long per = (R + k.splits - 1) / k.splits;
   r_begin = (long)sp * per; r_end = min(R, r_begin + per);
-  float acc[8];
+  float acc[HW];
 #pragma unroll
-  for (int c = 0; c < 8; ++c) acc[c] = 0.f;
+  for (int c = 0; c < HW; ++c) acc[c] = 0.f;
   for (long r = r_begin + part; r < r_end; r += NPARTS) {
     const long t = r / k.B, b = r - t * k.B;
     const size_t row = ((size_t)t * k.N + i) * k.B + b;
     const float hv = k.h1[row * H + u];
-    const float4 d0 = *reinterpret_cast<const float4*>(k.dlv + row * 8);
-    const float4 d1 = *reinterpret_cast<const float4*>(k.dlv + row * 8 + 4);
-    acc[0] = fmaf(hv, d0.x, acc[0]); acc[1] = fmaf(hv, d0.y, acc[1]); acc[2] = fmaf(hv, d0.z, acc[2]); acc[3] = fmaf(hv, d0.w, acc[3]);
-    acc[4] = fmaf(hv, d1.x, acc[4]); acc[5] = fmaf(hv, d1.y, acc[5]); acc[6] = fmaf(hv, d1.z, acc[6]); acc[7] = fmaf(hv, d1.w, acc[7]);
-  }
 #pragma unroll
-  for (int c = 0; c < 8; ++c) red[part][u][c] = acc[c];
-  }
-  // bias sums (8) and one-hot sums (n_nbr x n_a): every thread strides over the rows, then a fixed-order
-  // block reduction (warp shuffle tree + per-warp partials summed in warp order)
-  constexpr int NX = 8 + NMARL_MAX_NBR * NMARL_MAX_NA;
-  float ex[NX];
-#pragma unroll
-  for (int c = 0; c < NX; ++c) ex[c] = 0.f;
-  const int n_extra = 8 + ag.n_nbr * k.n_a;
-  for (long r = r_begin + tid; r < r_end; r += 256) {
-    const long t = r / k.B, b = r - t * k.B;
-    const size_t row = ((size_t)t * k.N + i) * k.B + b;
-    const float4 d0 = *reinterpret_cast<const float4*>(k.dlv + row * 8);
-    const float4 d1 = *reinterpret_cast<const float4*>(k.dlv + row * 8 + 4);
-    const float dl[8] = {d0.x, d0.y, d0.z, d0.w, d1.x, d1.y, d1.z, d1.w};
-#pragma unroll
-    for (int c = 0; c < 8; ++c) ex[c] += dl[c];
-    const float dv = dl[k.n_a];
-#pragma unroll
-    for (int s = 0; s < NMARL_MAX_NBR; ++s) {
-      if (s < ag.n_nbr) {
-        const int a = k.act[((size_t)t * k.N + ag.nbr[s]) * k.B + b];
-#pragma unroll
-        for (int c = 0; c < NMARL_MAX_NA; ++c) ex[8 + s * NMARL_MAX_NA + c] += (c == a) ? dv : 0.f;
-      }
+    for (int q = 0; q < HW / 4; ++q) {
+      const float4 d4 = *reinterpret_cast<const float4*>(k.dlv + row * HW + 4 * q);
+      acc[4 * q] = fmaf(hv, d4.x, acc[4 * q]); acc[4 * q + 1] = fmaf(hv, d4.y, acc[4 * q + 1]);
+      acc[4 * q + 2] = fmaf(hv, d4.z, acc[4 * q + 2]); acc[4 * q + 3] = fmaf(hv, d4.w, acc[4 * q + 3]);
     }
   }
-  __shared__ float redx[8][NX];
 #pragma unroll
-  for (int c = 0; c < NX; ++c) {
-    float x = ex[c];
-    for (int o = 16; o > 0; o >>= 1) x += __shfl_xor_sync(0xffffffffu, x, o);
-    if ((tid & 31) == 0) redx[tid >> 5][c] = x;
+  for (int c = 0; c < HW; ++c) red[part][u][c] = acc[c];
+  }
+  // bias sums (HW) and one-hot sums (n_nbr x n_a, at stride HW): every thread strides over the rows, then a fixed-order
+  // block reduction (warp shuffle tree + per-warp partials summed in warp order).  The NX extras are taken in passes
+  // of NXP over the rows, so that a thread holds 40 accumulators at either head width.
+  constexpr int NX = HW + NMARL_MAX_NBR * HW, NXP = (HW == 8) ? NX : NX / 2;
+  static_assert(NX % NXP == 0, "extras passes");
+  __shared__ float redx[8][NX];
+  const int n_extra = HW + ag.n_nbr * k.n_a;
+#pragma unroll
+  for (int x0 = 0; x0 < NX; x0 += NXP) {
+    float ex[NXP];
+#pragma unroll
+    for (int c = 0; c < NXP; ++c) ex[c] = 0.f;
+    for (long r = r_begin + tid; r < r_end; r += 256) {
+      const long t = r / k.B, b = r - t * k.B;
+      const size_t row = ((size_t)t * k.N + i) * k.B + b;
+      float dl[HW];
+#pragma unroll
+      for (int q = 0; q < HW / 4; ++q) {
+        const float4 d4 = *reinterpret_cast<const float4*>(k.dlv + row * HW + 4 * q);
+        dl[4 * q] = d4.x; dl[4 * q + 1] = d4.y; dl[4 * q + 2] = d4.z; dl[4 * q + 3] = d4.w;
+      }
+#pragma unroll
+      for (int c = 0; c < HW; ++c)
+        if (c >= x0 && c < x0 + NXP) ex[c - x0] += dl[c];
+      const float dv = dl[k.n_a];
+#pragma unroll
+      for (int s = 0; s < NMARL_MAX_NBR; ++s) {
+        if (HW + (s + 1) * HW <= x0 || HW + s * HW >= x0 + NXP) continue;     // slot outside this pass
+        if (s < ag.n_nbr) {
+          const int a = k.act[((size_t)t * k.N + ag.nbr[s]) * k.B + b];
+#pragma unroll
+          for (int c = 0; c < HW; ++c) {
+            const int e = HW + s * HW + c;
+            if (e >= x0 && e < x0 + NXP) ex[e - x0] += (c == a) ? dv : 0.f;
+          }
+        }
+      }
+    }
+#pragma unroll
+    for (int c = 0; c < NXP; ++c) {
+      float x = ex[c];
+      for (int o = 16; o > 0; o >>= 1) x += __shfl_xor_sync(0xffffffffu, x, o);
+      if ((tid & 31) == 0) redx[tid >> 5][x0 + c] = x;
+    }
   }
   __syncthreads();
   float extra = 0.f;
   if (tid < n_extra) {
-    const int src = tid < 8 ? tid : 8 + ((tid - 8) / k.n_a) * NMARL_MAX_NA + (tid - 8) % k.n_a;
+    const int src = tid < HW ? tid : HW + ((tid - HW) / k.n_a) * HW + (tid - HW) % k.n_a;
     for (int w2 = 0; w2 < 8; ++w2) extra += redx[w2][src];
   }
   red2[tid] = extra;
   __syncthreads();
-  float* w = k.ws + ((size_t)sp * k.N + i) * HEAD_WS;
-  for (int e = tid; e < H * 8; e += 256) {
-    const int uu = e >> 3, c = e & 7;
+  float* w = k.ws + ((size_t)sp * k.N + i) * head_ws(HW);
+  for (int e = tid; e < H * HW; e += 256) {
+    const int uu = e >> nmarl_log2(HW), c = e & (HW - 1);
     float x = red[0][uu][c];
 #pragma unroll
     for (int p = 1; p < NPARTS; ++p) x += red[p][uu][c];
     w[e] = x;
   }
-  if (tid < n_extra) w[H * 8 + tid] = red2[tid];
+  if (tid < n_extra) w[H * HW + tid] = red2[tid];
 }
 
 struct HeadRedK { int N, splits, n_a; const float* ws; float* grads; };
 
+template <int HW>
 __global__ void head_reduce_kernel(const __grid_constant__ nmarl_model m, const __grid_constant__ HeadRedK k) {
   const int i = blockIdx.x;
   const nmarl_agent& ag = m.agent[i];
-  const int n_extra = 8 + ag.n_nbr * k.n_a, H = nmarl_n_h(m);
-  for (int e = threadIdx.x; e < H * 8 + n_extra; e += blockDim.x) {
+  const int n_extra = HW + ag.n_nbr * k.n_a, H = nmarl_n_h(m);
+  for (int e = threadIdx.x; e < H * HW + n_extra; e += blockDim.x) {
     float s = 0.f;
-    for (int sp = 0; sp < k.splits; ++sp) s += k.ws[((size_t)sp * k.N + i) * HEAD_WS + e];
-    if (e < H * 8) {
-      const int u = e >> 3, c = e & 7;
+    for (int sp = 0; sp < k.splits; ++sp) s += k.ws[((size_t)sp * k.N + i) * head_ws(HW) + e];
+    if (e < H * HW) {
+      const int u = e >> nmarl_log2(HW), c = e & (HW - 1);
       if (c < k.n_a) k.grads[ag.o_pi_w + u * k.n_a + c] = s;
       else if (c == k.n_a) k.grads[ag.o_v_w + u] = s;
     } else {
-      const int x = e - H * 8;
+      const int x = e - H * HW;
       if (x < k.n_a) k.grads[ag.o_pi_b + x] = s;
       else if (x == k.n_a) k.grads[ag.o_v_b] = s;
-      else if (x >= 8) k.grads[ag.o_v_w + H + (x - 8)] = s;
+      else if (x >= HW) k.grads[ag.o_v_w + H + (x - HW)] = s;
     }
   }
+}
+
+template <int HW>
+int launch_head_wgrad(const nmarl_model* m, const HeadK& h, int H, float* grads, cudaStream_t st) {
+  const dim3 grid(h.splits, h.N);
+  switch (H) {
+    case 16: head_wgrad_kernel<16, HW><<<grid, 256, 0, st>>>(*m, h); break;
+    case 32: head_wgrad_kernel<32, HW><<<grid, 256, 0, st>>>(*m, h); break;
+    default: head_wgrad_kernel<64, HW><<<grid, 256, 0, st>>>(*m, h); break;
+  }
+  NMARL_LAUNCH_CHECK();
+  HeadRedK r{h.N, h.splits, m->n_a, h.ws, grads};
+  head_reduce_kernel<HW><<<h.N, 256, 0, st>>>(*m, r);
+  NMARL_LAUNCH_CHECK();
+  return 0;
 }
 
 // ============================ K10: clip + RMSProp ================================================
@@ -704,7 +753,7 @@ struct HeadFwdK {                 // pointers are for step 0; t = t0 + blockIdx.
   float loss_scale, v_coef, e_coef;
 };
 
-template <int H>
+template <int H, int HW>
 __global__ void __launch_bounds__(128) train_heads_kernel(const __grid_constant__ nmarl_model m, const __grid_constant__ HeadFwdK k) {
   __shared__ float red[3][4];
   const int i = blockIdx.y, b = blockIdx.x * 128 + threadIdx.x, B = k.B, t = k.t0 + blockIdx.z;
@@ -715,9 +764,9 @@ __global__ void __launch_bounds__(128) train_heads_kernel(const __grid_constant_
   const size_t tb = (size_t)t * k.N * B;                    // step offset in rows
   if (b < B) {
     const size_t row = tb + (size_t)i * B + b;
-    float logit[NMARL_MAX_NA];
+    float logit[HW];
 #pragma unroll
-    for (int cc = 0; cc < NMARL_MAX_NA; ++cc) logit[cc] = 0.f;
+    for (int cc = 0; cc < HW; ++cc) logit[cc] = 0.f;
     float v = 0.f;
 #pragma unroll 4
     for (int q = 0; q < H / 4; ++q) {
@@ -739,31 +788,31 @@ __global__ void __launch_bounds__(128) train_heads_kernel(const __grid_constant_
           logit[2] = fmaf(hv, w4.z, logit[2]); logit[3] = fmaf(hv, w4.w, logit[3]);
         } else {
 #pragma unroll
-          for (int cc = 0; cc < NMARL_MAX_NA; ++cc)
+          for (int cc = 0; cc < HW; ++cc)
             if (cc < n_a) logit[cc] = fmaf(hv, __ldg(P + ag.o_pi_w + u * n_a + cc), logit[cc]);
         }
         v = fmaf(hv, f4get(vw, j), v);
       }
     }
-    float pi[NMARL_MAX_NA];
+    float pi[HW];
     float mx = -3.0e38f;
 #pragma unroll
-    for (int cc = 0; cc < NMARL_MAX_NA; ++cc)
+    for (int cc = 0; cc < HW; ++cc)
       if (cc < n_a) { logit[cc] += __ldg(P + ag.o_pi_b + cc); mx = fmaxf(mx, logit[cc]); }
     float se = 0.f;
 #pragma unroll
-    for (int cc = 0; cc < NMARL_MAX_NA; ++cc)
+    for (int cc = 0; cc < HW; ++cc)
       if (cc < n_a) { pi[cc] = expf(logit[cc] - mx); se += pi[cc]; } else pi[cc] = 0.f;
 #pragma unroll
-    for (int cc = 0; cc < NMARL_MAX_NA; ++cc) if (cc < n_a) pi[cc] = pi[cc] / se;
+    for (int cc = 0; cc < HW; ++cc) if (cc < n_a) pi[cc] = pi[cc] / se;
     for (int s = 0; s < ag.n_nbr; ++s) v += __ldg(P + ag.o_v_w + H + s * n_a + k.act[tb + (size_t)ag.nbr[s] * B + b]);
     v += __ldg(P + ag.o_v_b);
     const int act = k.act[row];
     const float R = k.Rs[row], Adv = k.Advs[row], cs = k.loss_scale;
-    float g[NMARL_MAX_NA];
+    float g[HW];
     float ent = 0.f, dot = 0.f, lpa = 0.f;
 #pragma unroll
-    for (int cc = 0; cc < NMARL_MAX_NA; ++cc) {
+    for (int cc = 0; cc < HW; ++cc) {
       g[cc] = 0.f;
       if (cc < n_a) {
         const float pc = fminf(fmaxf(pi[cc], 1e-10f), 1.0f);
@@ -775,14 +824,15 @@ __global__ void __launch_bounds__(128) train_heads_kernel(const __grid_constant_
         dot += pi[cc] * g[cc];
       }
     }
-    float dl[8];
+    float dl[HW];
 #pragma unroll
-    for (int cc = 0; cc < 8; ++cc) dl[cc] = (cc < n_a) ? pi[cc] * (g[cc] - dot) : 0.f;
+    for (int cc = 0; cc < HW; ++cc) dl[cc] = (cc < n_a) ? pi[cc] * (g[cc] - dot) : 0.f;
     const float dvv = -k.v_coef * cs * (R - v);
 #pragma unroll
-    for (int cc = 0; cc < 8; ++cc) if (cc == n_a) dl[cc] = dvv;
-    *reinterpret_cast<float4*>(k.sv_dlv + row * 8) = make_float4(dl[0], dl[1], dl[2], dl[3]);
-    *reinterpret_cast<float4*>(k.sv_dlv + row * 8 + 4) = make_float4(dl[4], dl[5], dl[6], dl[7]);
+    for (int cc = 0; cc < HW; ++cc) if (cc == n_a) dl[cc] = dvv;
+#pragma unroll
+    for (int q = 0; q < HW / 4; ++q)
+      *reinterpret_cast<float4*>(k.sv_dlv + row * HW + 4 * q) = make_float4(dl[4 * q], dl[4 * q + 1], dl[4 * q + 2], dl[4 * q + 3]);
     l_pol = -lpa * Adv; l_val = (R - v) * (R - v); l_ent = ent;
   }
   float vals[3] = {l_pol, l_val, l_ent};
@@ -803,10 +853,10 @@ __global__ void __launch_bounds__(128) train_heads_kernel(const __grid_constant_
 
 constexpr int BWD_BM = 64;
 
-template <int VAR, int H>
+template <int VAR, int H, int HW>
 int launch_bwd(const nmarl_model* m, const BwdK& k, cudaStream_t st) {
   constexpr int NGRP = (VAR == NMARL_NC) ? 4 : 2, TY = nmarl_ffma_ty(H);
-  auto kern = cell_bwd_kernel<VAR, BWD_BM, TY, H>;
+  auto kern = cell_bwd_kernel<VAR, BWD_BM, TY, H, HW>;
   const size_t smem = ((size_t)BWD_BM * (4 * H + 4) + 2 * 16 * H * NGRP) * sizeof(float);
   static bool configured = false;
   if (!configured) {
@@ -819,15 +869,20 @@ int launch_bwd(const nmarl_model* m, const BwdK& k, cudaStream_t st) {
   return 0;
 }
 
-template <int VAR>
+template <int VAR, int HW>
 int launch_bwd_width(const nmarl_model* m, const BwdK& k, cudaStream_t st) {
   switch (nmarl_n_h(*m)) {
-    case 16: return launch_bwd<VAR, 16>(m, k, st);
-    case 32: return launch_bwd<VAR, 32>(m, k, st);
-    case 64: return launch_bwd<VAR, 64>(m, k, st);
+    case 16: return launch_bwd<VAR, 16, HW>(m, k, st);
+    case 32: return launch_bwd<VAR, 32, HW>(m, k, st);
+    case 64: return launch_bwd<VAR, 64, HW>(m, k, st);
   }
   nmarl_set_error("n_h %d has no FFMA kernel", nmarl_n_h(*m));
   return 1;
+}
+
+template <int VAR>
+int launch_bwd_head(const nmarl_model* m, const BwdK& k, cudaStream_t st) {
+  return nmarl_head_width(m->n_a) == 8 ? launch_bwd_width<VAR, 8>(m, k, st) : launch_bwd_width<VAR, 16>(m, k, st);
 }
 
 int launch_dial_msg_bwd(const nmarl_model* m, int B, const float* wt, const float* msg_t, const float* dmsg, float* sv_dmp,
@@ -944,7 +999,7 @@ extern "C" int64_t nmarl_ws_floats(const nmarl_model* m, int B, int T) {
   const int splits = wgrad_splits((long)B * T), H = nmarl_n_h(*m);
   int64_t gate = (int64_t)splits * m->n_agent * (m->s_dim + H + 1) * (4 * H);
   int64_t enc = (int64_t)splits * m->n_agent * (m->km_pad + m->kx_pad + 1) * H;
-  int64_t head = (int64_t)head_splits((long)B * T) * m->n_agent * HEAD_WS;
+  int64_t head = (int64_t)head_splits((long)B * T) * m->n_agent * head_ws(nmarl_head_width(m->n_a));
   int64_t r = gate > enc ? gate : enc;
   r = r > head ? r : head;
   const int64_t tcw = nmarl_tc_wgrad_ws_floats(m);
@@ -988,7 +1043,7 @@ extern "C" int nmarl_a2c_train_forward(const nmarl_model* m, const nmarl_bwd_arg
     int rc = nmarl_launch_train_fwd(m, &f, a->Rs + (size_t)t * nb, a->Advs + (size_t)t * nb,
                                     a->sv_xin + (size_t)t * nb * LDI, a->sv_sh + (size_t)t * nb * (m->s_dim + H),
                                     a->sv_gates + (size_t)t * nb * (4 * H), a->sv_enc ? a->sv_enc + (size_t)t * nb * (2 * H) : nullptr,
-                                    a->sv_dlv + (size_t)t * nb * 8, a->loss_part + (size_t)t * N * tiles * 4, scale,
+                                    a->sv_dlv + (size_t)t * nb * nmarl_head_width(m->n_a), a->loss_part + (size_t)t * N * tiles * 4, scale,
                                     a->v_coef, a->e_coef, st);
     if (rc) return rc;
   }
@@ -1007,10 +1062,11 @@ static int launch_train_heads(const nmarl_model* m, const nmarl_bwd_args* a, int
   k.sv_dlv = a->sv_dlv; k.loss_part = a->loss_part;
   k.loss_scale = 1.0f / ((float)T * (float)a->B_total); k.v_coef = a->v_coef; k.e_coef = a->e_coef;
   const dim3 grid((B + 127) / 128, N, nt);
+  const bool wide = nmarl_head_width(m->n_a) == 16;
   switch (nmarl_n_h(*m)) {
-    case 16: train_heads_kernel<16><<<grid, 128, 0, st>>>(*m, k); break;
-    case 32: train_heads_kernel<32><<<grid, 128, 0, st>>>(*m, k); break;
-    default: train_heads_kernel<64><<<grid, 128, 0, st>>>(*m, k); break;
+    case 16: (wide ? train_heads_kernel<16, 16> : train_heads_kernel<16, 8>)<<<grid, 128, 0, st>>>(*m, k); break;
+    case 32: (wide ? train_heads_kernel<32, 16> : train_heads_kernel<32, 8>)<<<grid, 128, 0, st>>>(*m, k); break;
+    default: (wide ? train_heads_kernel<64, 16> : train_heads_kernel<64, 8>)<<<grid, 128, 0, st>>>(*m, k); break;
   }
   NMARL_LAUNCH_CHECK();
   return 0;
@@ -1060,16 +1116,9 @@ extern "C" int nmarl_a2c_bptt(const nmarl_model* m, const nmarl_bwd_args* a, voi
     HeadK h{};
     h.N = N; h.B = B; h.T = T; h.splits = head_splits((long)B * T); h.n_a = m->n_a; h.fm = a->state_fm;
     h.h1 = a->h_seq + nb * H; h.dlv = a->sv_dlv; h.act = a->act; h.ws = a->ws;
-    NMARL_CHECK((int64_t)h.splits * N * HEAD_WS <= a->ws_floats, "head wgrad: workspace too small");
-    switch (H) {
-      case 16: head_wgrad_kernel<16><<<dim3(h.splits, N), 256, 0, side>>>(*m, h); break;
-      case 32: head_wgrad_kernel<32><<<dim3(h.splits, N), 256, 0, side>>>(*m, h); break;
-      default: head_wgrad_kernel<64><<<dim3(h.splits, N), 256, 0, side>>>(*m, h); break;
-    }
-    NMARL_LAUNCH_CHECK();
-    HeadRedK r{N, h.splits, m->n_a, a->ws, a->grads};
-    head_reduce_kernel<<<N, 256, 0, side>>>(*m, r);
-    NMARL_LAUNCH_CHECK();
+    const int hw = nmarl_head_width(m->n_a);
+    NMARL_CHECK((int64_t)h.splits * N * head_ws(hw) <= a->ws_floats, "head wgrad: workspace too small");
+    if ((hw == 8 ? launch_head_wgrad<8>(m, h, H, a->grads, side) : launch_head_wgrad<16>(m, h, H, a->grads, side))) return 1;
   }
   NMARL_CUDA(cudaEventRecord(ev_join, side));
   // 2. reverse time
@@ -1082,7 +1131,7 @@ extern "C" int nmarl_a2c_bptt(const nmarl_model* m, const nmarl_bwd_args* a, voi
     k.sv_gates = a->sv_gates + (size_t)t * nb * (4 * H);
     k.sv_sh = a->sv_sh + (size_t)t * nb * (SD + H);
     k.sv_enc = a->sv_enc ? a->sv_enc + (size_t)t * nb * (2 * H) : nullptr;
-    k.sv_dlv = a->sv_dlv + (size_t)t * nb * 8;
+    k.sv_dlv = a->sv_dlv + (size_t)t * nb * nmarl_head_width(m->n_a);
     k.c_prev = a->c_seq + (size_t)t * nb * H;
     k.c_cur = a->c_seq + (size_t)(t + 1) * nb * H;
     const int pin = (t + 1) & 1, pout = t & 1;
@@ -1107,10 +1156,10 @@ extern "C" int nmarl_a2c_bptt(const nmarl_model* m, const nmarl_bwd_args* a, voi
     if (use_tc) rc = nmarl_tc_launch_bwd(m, k, st);
     else
     switch (m->variant) {
-      case NMARL_IA2C: rc = launch_bwd_width<NMARL_IA2C>(m, k, st); break;
-      case NMARL_NC: rc = launch_bwd_width<NMARL_NC>(m, k, st); break;
-      case NMARL_IC3: rc = launch_bwd_width<NMARL_IC3>(m, k, st); break;
-      case NMARL_DIAL: rc = launch_bwd_width<NMARL_DIAL>(m, k, st); break;
+      case NMARL_IA2C: rc = launch_bwd_head<NMARL_IA2C>(m, k, st); break;
+      case NMARL_NC: rc = launch_bwd_head<NMARL_NC>(m, k, st); break;
+      case NMARL_IC3: rc = launch_bwd_head<NMARL_IC3>(m, k, st); break;
+      case NMARL_DIAL: rc = launch_bwd_head<NMARL_DIAL>(m, k, st); break;
     }
     if (rc) return rc;
     if (a->ev_step) NMARL_CUDA(cudaEventRecord((cudaEvent_t)a->ev_step[2 * t + 1], st));

@@ -81,7 +81,7 @@ class ModelLayout:
         if N > L.MAX_AGENT:
             raise ValueError('n_agent %d > %d' % (N, L.MAX_AGENT))
         if not 0 < n_a < L.MAX_NA:
-            raise ValueError('n_a %d out of range' % n_a)
+            raise ValueError('n_a %d out of range (1..%d actions)' % (n_a, L.MAX_NA - 1))
         self.N, self.n_a, self.mask = N, int(n_a), mask
         self.nbr = [list(map(int, np.where(mask[i] == 1)[0])) for i in range(N)]
         if max(len(x) for x in self.nbr) > L.MAX_NBR:

@@ -35,7 +35,8 @@ extern "C" {
 /* LSTM width the tensor-core kernels are built for (num_lstm = 64 in every shipped config).  The FP32-FFMA kernels
  * also run n_h = 16 and 32 (n_h follows from nmarl_model.s_dim); any other model never takes the tensor-core path. */
 #define NMARL_NH        64
-#define NMARL_MAX_NA    8
+/* n_a <= NMARL_MAX_NA - 1 = 15: the n_a logits and the value slot of a row fill at most 16 head columns (DESIGN 4.8) */
+#define NMARL_MAX_NA    16
 
 enum { NMARL_IA2C = 0, NMARL_NC = 1, NMARL_IC3 = 2, NMARL_DIAL = 3 };
 enum { NMARL_SAMPLE_NONE = 0, NMARL_SAMPLE_UNIFORM = 1, NMARL_SAMPLE_PHILOX = 2, NMARL_SAMPLE_GREEDY = 3 };
@@ -208,7 +209,9 @@ int nmarl_nstep_return_adv(int n_agent, int B, int T, int NR, const double* rewa
  *   h_seq, c_seq [T+1][N][B][64]  (index 0 = states_bw, filled by the caller)
  *   msg_seq      [T+1][N][B][64]  (DIAL; index 0 filled by nmarl_dial_msg)
  *   sv_xin [T][N][B][kx_pad+kp_pad+km_pad]  sv_sh [T][N][B][s_dim+64]  sv_gates [T][N][B][256]
- *   sv_enc [T][N][B][2*n_h] (IC3: n_h used; DIAL: 2*n_h)   sv_dlv [T][N][B][8]
+ *   sv_enc [T][N][B][2*n_h] (IC3: n_h used; DIAL: 2*n_h)   sv_dlv [T][N][B][HW]
+ *   (head width HW = 8 for n_a <= 7, 16 for n_a 8..15: a row holds d(loss)/d(logits) in columns [0, n_a),
+ *    d(loss)/d(v) in column n_a and zeros behind it)
  *   sv_dz [T][N][B][4*n_h]   sv_dpre [T][N][B][3*n_h]   sv_dmp [T][N][B][n_h] (DIAL)
  *   (the widths written 64 / 256 / 192 in this block are n_h / 4*n_h / 3*n_h; the tensor-core path has n_h = 64)
  *   (tensor-core path: sv_dz = [T][N][B/32][256] gate-bias partial sums per 32 rows, sv_dpre unused)
