@@ -399,7 +399,6 @@ class PolicyEngine:
         a = self._bwd_args(T)
         if getattr(self, 'saved_rollout', False):
             # activations, h_seq / c_seq (slot 0 == states_bw) were written by the rollout p-calls
-            a.fused_heads = 1        # heads / loss kernel folded into the BPTT call (side stream, beside the first steps)
             L.check(L.lib().nmarl_a2c_bptt(C.byref(self.model), C.byref(a), L.stream()), 'nmarl_a2c_bptt')
             self.launches += 2 * T + 16
             self.saved_rollout = False

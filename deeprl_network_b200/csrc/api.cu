@@ -14,8 +14,9 @@ void nmarl_set_error(const char* fmt, ...) {
 
 extern "C" const char* nmarl_last_error(void) { return g_err; }
 // 101: NMARL_MAX_AGENT 32 -> 128; 102: n_h = 16 / 32 (s_dim); 103: nmarl_eval_record; 104: n_a up to 15 (sv_dlv rows
-// are nmarl_head_width(n_a) floats wide)
-extern "C" int nmarl_version(void) { return 104; }
+// are nmarl_head_width(n_a) floats wide); 105: nmarl_a2c_bptt always computes the heads; the bwd_args field and the
+// entry point that chose whether it did are gone
+extern "C" int nmarl_version(void) { return 105; }
 extern "C" int nmarl_sizeof_model(void) { return (int)sizeof(nmarl_model); }
 extern "C" int nmarl_sizeof_agent(void) { return (int)sizeof(nmarl_agent); }
 extern "C" int nmarl_sizeof_cacc_cfg(void) { return (int)sizeof(nmarl_cacc_cfg); }

@@ -10,7 +10,8 @@
 // Restates (per agent i, gate order i,f,o,u, state [c|h]):
 //   lstm_comm  agents/utils.py:163-217      lstm_ic3  :378-417      lstm_dial :555-599
 //   lstm (IA2C) :87-115 + fc policies.py:145   heads policies.py:50-77   sampling utils.py:135-141
-//   A2C loss terms policies.py:236-255 (TRAIN mode: per-row loss + d/dlogits, d/dv)
+// MODE_PS is the p-call that also saves the activations BPTT needs (a.sv_*, row-major [N][B][..] on this path);
+// the training forward runs it with sampling off.  The A2C loss head is train_heads_kernel (train.cu).
 #include "cell_common.cuh"
 
 namespace {
@@ -34,6 +35,8 @@ __global__ void __launch_bounds__(H / 4 * TY) cell_fwd_kernel(const __grid_const
   constexpr int NT = H / 4 * TY, TM = BM / TY, KC = 16;
   static_assert(BM % TY == 0 && NT >= BM, "tile/thread mismatch");
   extern __shared__ __align__(16) float smem[];
+  constexpr bool SAVE = (MODE == MODE_PS);                         // store activations for BPTT
+  constexpr bool SAMPLE = (MODE == MODE_P || MODE == MODE_PS);     // p-call: sample actions
   const nmarl_fwd_args& a = k.a;
   const int i = blockIdx.y;
   const nmarl_agent& ag = m.agent[i];
@@ -112,11 +115,11 @@ __global__ void __launch_bounds__(H / 4 * TY) cell_fwd_kernel(const __grid_const
     *reinterpret_cast<float4*>(SH + r * LDS + SD + 4 * u4) = v;
   }
   __syncthreads();
-  if (MODE == MODE_TRAIN) {                                            // save gathered inputs for wgrad
+  if (SAVE) {                                                          // save gathered inputs for wgrad
     const int q4 = LDI / 4;
     for (int idx = tid; idx < rows * q4; idx += NT) {
       const int r = idx / q4, c4 = idx - r * q4;
-      *reinterpret_cast<float4*>(k.sv_xin + ((size_t)i * B + b0 + r) * LDI + 4 * c4) =
+      *reinterpret_cast<float4*>(a.sv_xin + ((size_t)i * B + b0 + r) * LDI + 4 * c4) =
           *reinterpret_cast<const float4*>(IN + r * LDI + 4 * c4);
     }
   }
@@ -137,8 +140,8 @@ __global__ void __launch_bounds__(H / 4 * TY) cell_fwd_kernel(const __grid_const
       const int r = ty + TY * q;
       if (VAR == NMARL_NC || VAR == NMARL_IA2C)
         *reinterpret_cast<float4*>(SH + r * LDS + 4 * tx) = make_float4(sv[q][0], sv[q][1], sv[q][2], sv[q][3]);
-      if (MODE == MODE_TRAIN && (VAR == NMARL_IC3 || VAR == NMARL_DIAL) && r < rows)
-        *reinterpret_cast<float4*>(k.sv_enc + ((size_t)i * B + b0 + r) * (2 * H) + 4 * tx) =
+      if (SAVE && (VAR == NMARL_IC3 || VAR == NMARL_DIAL) && r < rows)
+        *reinterpret_cast<float4*>(a.sv_enc + ((size_t)i * B + b0 + r) * (2 * H) + 4 * tx) =
             make_float4(sv[q][0], sv[q][1], sv[q][2], sv[q][3]);
     }
   }
@@ -187,8 +190,8 @@ __global__ void __launch_bounds__(H / 4 * TY) cell_fwd_kernel(const __grid_const
 #pragma unroll
         for (int j = 0; j < 4; ++j) o[j] = (sv[q][j] + hm[j]) + ((4 * tx + j) == am ? 1.0f : 0.0f);
         *reinterpret_cast<float4*>(SH + r * LDS + 4 * tx) = make_float4(o[0], o[1], o[2], o[3]);
-        if (MODE == MODE_TRAIN && r < rows)
-          *reinterpret_cast<float4*>(k.sv_enc + ((size_t)i * B + b0 + r) * (2 * H) + H + 4 * tx) =
+        if (SAVE && r < rows)
+          *reinterpret_cast<float4*>(a.sv_enc + ((size_t)i * B + b0 + r) * (2 * H) + H + 4 * tx) =
               make_float4(hm[0], hm[1], hm[2], hm[3]);
       }
     }
@@ -202,11 +205,11 @@ __global__ void __launch_bounds__(H / 4 * TY) cell_fwd_kernel(const __grid_const
 #pragma unroll
     for (int c = 0; c < 16; ++c) acc[q][c] = 0.f;
   gemm_rowA<TM, 4, TY, KC, H>(acc, SH, LDS, SD + H, P + ag.o_wxh, (4 * H), WsG, tid);
-  if (MODE == MODE_TRAIN) {                                             // save [s | h^] for wgrad
+  if (SAVE) {                                                          // save [s | h^] for wgrad
     const int q4 = (SD + H) / 4;
     for (int idx = tid; idx < rows * q4; idx += NT) {
       const int r = idx / q4, c4 = idx - r * q4;
-      *reinterpret_cast<float4*>(k.sv_sh + ((size_t)i * B + b0 + r) * (SD + H) + 4 * c4) =
+      *reinterpret_cast<float4*>(a.sv_sh + ((size_t)i * B + b0 + r) * (SD + H) + 4 * c4) =
           *reinterpret_cast<const float4*>(SH + r * LDS + 4 * c4);
     }
   }
@@ -237,8 +240,8 @@ __global__ void __launch_bounds__(H / 4 * TY) cell_fwd_kernel(const __grid_const
           *reinterpret_cast<float4*>(a.c_out + row * H + 4 * tx) = make_float4(cn[0], cn[1], cn[2], cn[3]);
           *reinterpret_cast<float4*>(a.h_out + row * H + 4 * tx) = make_float4(hn[0], hn[1], hn[2], hn[3]);
         }
-        if (MODE == MODE_TRAIN) {
-          float* gs = k.sv_gates + row * (4 * H) + 4 * tx;
+        if (SAVE) {
+          float* gs = a.sv_gates + row * (4 * H) + 4 * tx;
           *reinterpret_cast<float4*>(gs + 0 * H) = make_float4(gi[0], gi[1], gi[2], gi[3]);
           *reinterpret_cast<float4*>(gs + 1 * H) = make_float4(gf[0], gf[1], gf[2], gf[3]);
           *reinterpret_cast<float4*>(gs + 2 * H) = make_float4(go[0], go[1], go[2], go[3]);
@@ -251,7 +254,6 @@ __global__ void __launch_bounds__(H / 4 * TY) cell_fwd_kernel(const __grid_const
   __syncthreads();
 
   // ---- phase 3: heads (one thread per env row) ------------------------------------------------
-  float l_pol = 0.f, l_val = 0.f, l_ent = 0.f;
   if (tid < rows) {
     const int r = tid, b = b0 + r;
     const size_t row = (size_t)i * B + b;
@@ -278,7 +280,7 @@ __global__ void __launch_bounds__(H / 4 * TY) cell_fwd_kernel(const __grid_const
       if (a.pi != nullptr)
         for (int c = 0; c < n_a; ++c) a.pi[row * n_a + c] = pi[c];
     }
-    if (MODE == MODE_P && a.action != nullptr && a.sample_mode != NMARL_SAMPLE_NONE) {
+    if (SAMPLE && a.action != nullptr && a.sample_mode != NMARL_SAMPLE_NONE) {
       int act = 0;
       if (a.sample_mode == NMARL_SAMPLE_GREEDY) {                       // np.argmax: first maximum
         float best = pi[0];
@@ -295,51 +297,13 @@ __global__ void __launch_bounds__(H / 4 * TY) cell_fwd_kernel(const __grid_const
       }
       a.action[row] = act;
     }
-    float v = 0.f;
-    if (MODE != MODE_P) {                                               // v = [h, onehot(a_j)] W_v + b  (policies.py:59-77)
+    if (!SAMPLE) {                                                      // v = [h, onehot(a_j)] W_v + b  (policies.py:59-77)
+      float v = 0.f;
 #pragma unroll
       for (int u = 0; u < H; ++u) v = fmaf(h[u], __ldg(P + ag.o_v_w + u), v);
       for (int s = 0; s < ag.n_nbr; ++s) v += __ldg(P + ag.o_v_w + H + s * n_a + a.act_in[(size_t)ag.nbr[s] * B + b]);
       v += __ldg(P + ag.o_v_b);
       if (a.v != nullptr) a.v[row] = v;
-    }
-    if (MODE == MODE_TRAIN) {
-      const int act = a.act_in[row];
-      const float R = k.Rs[row], Adv = k.Advs[row];
-      const float cs = k.loss_scale;
-      float lp[HW], g[HW];
-      float ent = 0.f, dot = 0.f;
-      for (int c = 0; c < n_a; ++c) {
-        const float pc = fminf(fmaxf(pi[c], 1e-10f), 1.0f);
-        const float in_rng = (pi[c] >= 1e-10f && pi[c] <= 1.0f) ? 1.0f : 0.0f;
-        lp[c] = logf(pc);
-        ent -= pi[c] * lp[c];
-        g[c] = k.e_coef * cs * (lp[c] + in_rng);
-        if (c == act) g[c] += -cs * Adv * in_rng / pc;
-      }
-      for (int c = 0; c < n_a; ++c) dot += pi[c] * g[c];
-      float* dl = k.sv_dlv + row * HW;
-      for (int c = 0; c < HW; ++c) dl[c] = (c < n_a) ? pi[c] * (g[c] - dot) : 0.f;
-      dl[n_a] = -k.v_coef * cs * (R - v);
-      l_pol = -lp[act] * Adv;
-      l_val = (R - v) * (R - v);
-      l_ent = ent;
-    }
-  }
-  if (MODE == MODE_TRAIN) {                                             // deterministic per-CTA loss partials
-    __shared__ float red[3][32];
-    float vals[3] = {l_pol, l_val, l_ent};
-#pragma unroll
-    for (int c = 0; c < 3; ++c) {
-      float x = vals[c];
-      for (int o = 16; o > 0; o >>= 1) x += __shfl_xor_sync(0xffffffffu, x, o);
-      if ((tid & 31) == 0) red[c][tid >> 5] = x;
-    }
-    __syncthreads();
-    if (tid < 3) {
-      float s = 0.f;
-      for (int w = 0; w < NT / 32; ++w) s += red[tid][w];
-      k.loss_part[((size_t)i * k.loss_tiles + blockIdx.x) * 4 + tid] = s;
     }
   }
   if (VAR == NMARL_DIAL && MODE != MODE_V) {                            // sender-side message of the NEW h (utils.py:563-566)
@@ -472,22 +436,14 @@ int check_model(const nmarl_model* m) {
 }  // namespace
 
 int nmarl_check_model(const nmarl_model* m) { return check_model(m); }
-int nmarl_fwd_tiles(int B) { return (B + 64 - 1) / 64; }
 
-int nmarl_fwd_tiles(int B);
-// entry used by train.cu for the TRAIN-mode forward of one time step
-int nmarl_launch_train_fwd(const nmarl_model* m, const nmarl_fwd_args* a, const float* Rs, const float* Advs,
-                           float* sv_xin, float* sv_sh, float* sv_gates, float* sv_enc, float* sv_dlv,
-                           float* loss_part, float loss_scale, float v_coef, float e_coef, cudaStream_t st) {
+// forward of one step that saves the activations BPTT needs (a->sv_*): the rollout's saving p-calls and the
+// training forward (train.cu)
+int nmarl_launch_save_fwd(const nmarl_model* m, const nmarl_fwd_args* a, cudaStream_t st) {
   FwdK k{};
   k.a = *a;
-  k.Rs = Rs; k.Advs = Advs;
-  k.sv_xin = sv_xin; k.sv_sh = sv_sh; k.sv_gates = sv_gates; k.sv_enc = sv_enc; k.sv_dlv = sv_dlv;
-  k.loss_part = loss_part; k.loss_tiles = nmarl_fwd_tiles(a->B); k.loss_scale = loss_scale; k.v_coef = v_coef; k.e_coef = e_coef;
-  return dispatch_fwd<MODE_TRAIN>(m, k, st);
+  return dispatch_fwd<MODE_PS>(m, k, st);
 }
-
-
 
 extern "C" int nmarl_policy_step_p(const nmarl_model* m, const nmarl_fwd_args* a, void* stream) {
   if (check_model(m)) return 1;
@@ -499,15 +455,14 @@ extern "C" int nmarl_policy_step_p(const nmarl_model* m, const nmarl_fwd_args* a
   NMARL_CHECK(a->sample_mode != NMARL_SAMPLE_UNIFORM || a->uniforms, "policy_step_p: uniforms required");
   NMARL_CHECK(a->sample_mode != NMARL_SAMPLE_PHILOX || a->rng, "policy_step_p: rng state required");
   NMARL_CHECK(!a->state_fm || nmarl_tc_fwd_supported(m, a), "policy_step_p: feature-major state needs the tensor-core path");
-  FwdK k{};
-  k.a = *a;
   if (a->sv_sh != nullptr) {                 // rollout p-call that also saves activations for BPTT
     NMARL_CHECK(nmarl_tc_fwd_supported(m, a), "policy_step_p: activation saving needs the tensor-core path (B %% 128 == 0, wpack)");
     NMARL_CHECK(a->sv_xin && a->sv_gates, "policy_step_p: sv_xin / sv_gates missing");
     NMARL_CHECK((m->variant != NMARL_IC3 && m->variant != NMARL_DIAL) || a->sv_enc, "policy_step_p: sv_enc missing");
-    k.sv_xin = a->sv_xin; k.sv_sh = a->sv_sh; k.sv_gates = a->sv_gates; k.sv_enc = a->sv_enc;
-    return nmarl_tc_launch_fwd(m, k, MODE_PS, (cudaStream_t)stream);
+    return nmarl_launch_save_fwd(m, a, (cudaStream_t)stream);
   }
+  FwdK k{};
+  k.a = *a;
   return dispatch_fwd<MODE_P>(m, k, (cudaStream_t)stream);
 }
 

@@ -29,13 +29,12 @@ using namespace tcrow;
 template <int VAR, int MODE, bool FM, int HW>
 __global__ void __launch_bounds__(TC_THREADS, 1) tc_cell_fwd_kernel(const __grid_constant__ nmarl_model m,
                                                                     const __grid_constant__ FwdK k) {
-  constexpr bool SAVE = (MODE == MODE_TRAIN || MODE == MODE_PS);   // store activations for BPTT
+  constexpr bool SAVE = (MODE == MODE_PS);                         // store activations for BPTT
   constexpr bool SAMPLE = (MODE == MODE_P || MODE == MODE_PS);     // p-call: sample actions
   static_assert(HW <= EW, "a set's HW partial head sums live in its EW gate-f staging columns");
   extern __shared__ uint8_t smem_raw[];
   const Smem sm = smem_map(smem_raw);
   KbEnt* sched = sm.sched;
-  __shared__ float red[3][ROW_WARPS];
 
   const nmarl_fwd_args& a = k.a;
   const int i = blockIdx.y;
@@ -86,10 +85,10 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_cell_fwd_kernel(const __grid
     const float nd = 1.0f - a.done[b];
     const int LDI = m.kx_pad + m.kp_pad + m.km_pad;
     // saved activations are feature-major on this path: [agent][feature][env]
-    float* xin_fm = SAVE ? k.sv_xin + (size_t)i * LDI * B : nullptr;
-    float* sh_fm = SAVE ? k.sv_sh + (size_t)i * (SD + NH) * B : nullptr;
-    float* enc_fm = (SAVE && k.sv_enc) ? k.sv_enc + (size_t)i * 128 * B : nullptr;
-    float* gates_fm = SAVE ? k.sv_gates + (size_t)i * NG * B : nullptr;
+    float* xin_fm = SAVE ? a.sv_xin + (size_t)i * LDI * B : nullptr;
+    float* sh_fm = SAVE ? a.sv_sh + (size_t)i * (SD + NH) * B : nullptr;
+    float* enc_fm = (SAVE && a.sv_enc) ? a.sv_enc + (size_t)i * 128 * B : nullptr;
+    float* gates_fm = SAVE ? a.sv_gates + (size_t)i * NG * B : nullptr;
     long long* prof = (k.prof != nullptr && blockIdx.x == 0 && blockIdx.y == 1 && tid == 0) ? k.prof : nullptr;
     int pi_ = 0;
 #define STAMP() do { if (prof) prof[pi_++] = clock64(); } while (0)
@@ -344,7 +343,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_cell_fwd_kernel(const __grid
     }
     if (VAR == NMARL_DIAL && MODE != MODE_V) produce_act(c, s0);
 
-    // ---- heads: combine the NSET partial sums of a row in fixed order, then softmax / sampling / loss -------
+    // ---- heads: combine the NSET partial sums of a row in fixed order, then softmax / sampling ---------------
     // The partial sums of set s go to staging columns [NH + s*EW, +HW) of the row (HW - 1 logits, then v): gate-f
     // cells that only this thread has read, and that the DIAL message GEMM (columns [0, NH)) does not overwrite.
     {
@@ -356,7 +355,6 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_cell_fwd_kernel(const __grid
     STAMP();
     row_barrier();
     STAMP();
-    float l_pol = 0.f, l_val = 0.f, l_ent = 0.f;
     if (set == 0) {
 #pragma unroll
       for (int cc = 0; cc < HW; ++cc) logit[cc] = 0.f;
@@ -416,36 +414,6 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_cell_fwd_kernel(const __grid
         v += __ldg(P + ag.o_v_b);
         if (a.v != nullptr) a.v[row] = v;
       }
-      if (MODE == MODE_TRAIN) {
-        const int act = a.act_in[row];
-        const float R = k.Rs[row], Adv = k.Advs[row];
-        const float cs = k.loss_scale;
-        float g[HW];
-        float ent = 0.f, dot = 0.f, lpa = 0.f;
-#pragma unroll
-        for (int cc = 0; cc < HW; ++cc) {
-          g[cc] = 0.f;
-          if (cc < n_a) {
-            const float pc = fminf(fmaxf(pi[cc], 1e-10f), 1.0f);
-            const float in_rng = (pi[cc] >= 1e-10f && pi[cc] <= 1.0f) ? 1.0f : 0.0f;
-            const float lp = logf(pc);
-            ent -= pi[cc] * lp;
-            g[cc] = k.e_coef * cs * (lp + in_rng);
-            if (cc == act) { g[cc] += -cs * Adv * in_rng / pc; lpa = lp; }
-            dot += pi[cc] * g[cc];
-          }
-        }
-        float dl[HW];
-#pragma unroll
-        for (int cc = 0; cc < HW; ++cc) dl[cc] = (cc < n_a) ? pi[cc] * (g[cc] - dot) : 0.f;
-        const float dvv = -k.v_coef * cs * (R - v);
-#pragma unroll
-        for (int cc = 0; cc < HW; ++cc) if (cc == n_a) dl[cc] = dvv;
-#pragma unroll
-        for (int q = 0; q < HW / 4; ++q)
-          *reinterpret_cast<float4*>(k.sv_dlv + row * HW + 4 * q) = make_float4(dl[4 * q], dl[4 * q + 1], dl[4 * q + 2], dl[4 * q + 3]);
-        l_pol = -lpa * Adv; l_val = (R - v) * (R - v); l_ent = ent;
-      }
     }
     if (VAR == NMARL_DIAL && MODE != MODE_V) {            // msg' = relu(h' W_mfc + b)   (utils.py:563-566)
       float mo[EW];
@@ -456,24 +424,11 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_cell_fwd_kernel(const __grid
     }
     STAMP();
     if (prof) prof[31] = pi_;
-    if (MODE == MODE_TRAIN && set == 0) {
-      float vals[3] = {l_pol, l_val, l_ent};
-#pragma unroll
-      for (int cc = 0; cc < 3; ++cc) {
-        float x = vals[cc];
-        for (int o = 16; o > 0; o >>= 1) x += __shfl_xor_sync(0xffffffffu, x, o);
-        if (lane == 0) red[cc][rh] = x;
-      }
-    }
   } else {
     // =================================== MMA warpgroup ===================================================
     mma_loop(sched, n_kb, sm.bst, sm.ast, sm.b_full, sm.a_full, sm.a_empty, sm.enc_full, sm.acc_full, sm.acc, a.wpack, a.tc_err);
   }
   __syncthreads();
-  if (MODE == MODE_TRAIN && tid < 3) {
-    static_assert(ROWS == 64 && ROW_WARPS == 2, "one 64-row loss tile per CTA");
-    k.loss_part[((size_t)i * k.loss_tiles + blockIdx.x) * 4 + tid] = red[tid][0] + red[tid][1];
-  }
 }
 
 
@@ -510,8 +465,7 @@ int launch_tc_mode(const nmarl_model* m, const FwdK& k, int mode, cudaStream_t s
   switch (mode) {
     case MODE_P: return launch_tc<VAR, MODE_P>(m, k, st);
     case MODE_V: return launch_tc<VAR, MODE_V>(m, k, st);
-    case MODE_PS: return launch_tc<VAR, MODE_PS>(m, k, st);
-    default: return launch_tc<VAR, MODE_TRAIN>(m, k, st);
+    default: return launch_tc<VAR, MODE_PS>(m, k, st);
   }
 }
 

@@ -3,8 +3,9 @@
 //
 // Backward structure (per update of T steps):
 //   1. transposed copies of [wx;wh], w_msg, w_mfc (once per update; weights only change in K10)
-//   2. T launches of the TRAIN-mode forward (cell_fwd.cu) saving activations + per-row
-//      d(loss)/d(logits,v)                                              (policies.py:232-255)
+//   2. T launches of the saving forward (cell_fwd.cu, MODE_PS without sampling), or none when the rollout
+//      p-calls already saved the activations; then train_heads_kernel: heads, loss partials and per-row
+//      d(loss)/d(logits,v) from h_seq                                   (policies.py:232-255)
 //   3. T reverse launches of cell_bwd_kernel: gate derivatives -> dgrad GEMM dz [wx;wh]^T ->
 //      encoder pre-activation grads -> message gradient dm = dpre_m W_msg^T written per
 //      (receiver, slot) and GATHERED by the sender at step t-1 (deterministic; the transpose of
@@ -13,10 +14,7 @@
 #include "bwd_common.cuh"
 
 int nmarl_check_model(const nmarl_model* m);
-int nmarl_launch_train_fwd(const nmarl_model* m, const nmarl_fwd_args* a, const float* Rs, const float* Advs,
-                           float* sv_xin, float* sv_sh, float* sv_gates, float* sv_enc, float* sv_dlv,
-                           float* loss_part, float loss_scale, float v_coef, float e_coef, cudaStream_t st);
-int nmarl_fwd_tiles(int B);
+int nmarl_launch_save_fwd(const nmarl_model* m, const nmarl_fwd_args* a, cudaStream_t st);
 
 namespace {
 
@@ -744,8 +742,9 @@ __global__ void __launch_bounds__(256) rmsprop_kernel(const __grid_constant__ Op
   }
 }
 
-// Heads + A2C loss terms + d(loss)/d(logits, v) from the saved h sequence (thread == env row); used when the
-// rollout already saved the cell activations.  Same arithmetic as the TRAIN epilogue of the forward kernels.
+// Heads + A2C loss terms + d(loss)/d(logits, v) from the saved h sequence (thread == env row).  Each sum runs in one
+// fixed order over ascending units, whichever forward kernel wrote h_seq.  loss_part gets one 128-row partial sum per
+// CTA, in the first of its two 64-row tiles; the second is zeroed.
 struct HeadFwdK {                 // pointers are for step 0; t = t0 + blockIdx.z strides them
   int B, N, loss_tiles, fm, t0;
   const float* params; const float* h1; const int32_t* act; const float* Rs; const float* Advs;
@@ -904,6 +903,8 @@ int wgrad_splits(long R) {
   return (int)s;
 }
 
+int loss_tiles(int B) { return (B + 64 - 1) / 64; }
+
 int head_splits(long R) {
   long s = R / 1024;
   if (s < 1) s = 1;
@@ -993,7 +994,7 @@ int nmarl_launch_transposes(const nmarl_model* m, int jobs, const float* params,
   return 0;
 }
 
-extern "C" int nmarl_loss_tiles(const nmarl_model* m, int B) { (void)m; return nmarl_fwd_tiles(B); }
+extern "C" int nmarl_loss_tiles(const nmarl_model* m, int B) { (void)m; return loss_tiles(B); }
 
 extern "C" int64_t nmarl_ws_floats(const nmarl_model* m, int B, int T) {
   const int splits = wgrad_splits((long)B * T), H = nmarl_n_h(*m);
@@ -1024,11 +1025,9 @@ extern "C" int nmarl_nstep_return_adv(int n_agent, int B, int T, int NR, const d
 extern "C" int nmarl_a2c_train_forward(const nmarl_model* m, const nmarl_bwd_args* a, void* stream) {
   if (check_bwd_args(m, a)) return 1;
   cudaStream_t st = (cudaStream_t)stream;
-  const int N = m->n_agent, B = a->B, T = a->T, H = nmarl_n_h(*m);
-  const size_t nb = (size_t)N * B;
+  const int B = a->B, T = a->T, H = nmarl_n_h(*m);
+  const size_t nb = (size_t)m->n_agent * B;
   const int LDI = m->kx_pad + m->kp_pad + m->km_pad;
-  const int tiles = nmarl_fwd_tiles(B);
-  const float scale = 1.0f / ((float)T * (float)a->B_total);
   for (int t = 0; t < T; ++t) {
     nmarl_fwd_args f{};
     f.B = B; f.params = a->params;
@@ -1038,14 +1037,12 @@ extern "C" int nmarl_a2c_train_forward(const nmarl_model* m, const nmarl_bwd_arg
     f.c_in = a->c_seq + (size_t)t * nb * H;       f.h_in = a->h_seq + (size_t)t * nb * H;
     f.c_out = a->c_seq + (size_t)(t + 1) * nb * H; f.h_out = a->h_seq + (size_t)(t + 1) * nb * H;
     if (m->variant == NMARL_DIAL) { f.msg_in = a->msg_seq + (size_t)t * nb * H; f.msg_out = a->msg_seq + (size_t)(t + 1) * nb * H; }
-    f.act_in = a->act + (size_t)t * nb;
+    f.sample_mode = NMARL_SAMPLE_NONE;
     f.wpack = a->wpack; f.tc_err = a->tc_err; f.state_fm = a->state_fm;
-    int rc = nmarl_launch_train_fwd(m, &f, a->Rs + (size_t)t * nb, a->Advs + (size_t)t * nb,
-                                    a->sv_xin + (size_t)t * nb * LDI, a->sv_sh + (size_t)t * nb * (m->s_dim + H),
-                                    a->sv_gates + (size_t)t * nb * (4 * H), a->sv_enc ? a->sv_enc + (size_t)t * nb * (2 * H) : nullptr,
-                                    a->sv_dlv + (size_t)t * nb * nmarl_head_width(m->n_a), a->loss_part + (size_t)t * N * tiles * 4, scale,
-                                    a->v_coef, a->e_coef, st);
-    if (rc) return rc;
+    f.sv_xin = a->sv_xin + (size_t)t * nb * LDI;  f.sv_sh = a->sv_sh + (size_t)t * nb * (m->s_dim + H);
+    f.sv_gates = a->sv_gates + (size_t)t * nb * (4 * H);
+    f.sv_enc = a->sv_enc ? a->sv_enc + (size_t)t * nb * (2 * H) : nullptr;
+    if (int rc = nmarl_launch_save_fwd(m, &f, st)) return rc;
   }
   return 0;
 }
@@ -1056,7 +1053,7 @@ static int launch_train_heads(const nmarl_model* m, const nmarl_bwd_args* a, int
   const int N = m->n_agent, B = a->B, T = a->T;
   const size_t nb = (size_t)N * B;
   HeadFwdK k{};
-  k.B = B; k.N = N; k.loss_tiles = nmarl_fwd_tiles(B); k.params = a->params; k.fm = a->state_fm; k.t0 = t0;
+  k.B = B; k.N = N; k.loss_tiles = loss_tiles(B); k.params = a->params; k.fm = a->state_fm; k.t0 = t0;
   k.h1 = a->h_seq + nb * nmarl_n_h(*m);                              // h after step t = h_seq[t + 1]
   k.act = a->act; k.Rs = a->Rs; k.Advs = a->Advs;
   k.sv_dlv = a->sv_dlv; k.loss_part = a->loss_part;
@@ -1070,11 +1067,6 @@ static int launch_train_heads(const nmarl_model* m, const nmarl_bwd_args* a, int
   }
   NMARL_LAUNCH_CHECK();
   return 0;
-}
-
-extern "C" int nmarl_a2c_train_heads(const nmarl_model* m, const nmarl_bwd_args* a, void* stream) {
-  if (check_bwd_args(m, a)) return 1;
-  return launch_train_heads(m, a, 0, a->T, (cudaStream_t)stream);
 }
 
 extern "C" int nmarl_a2c_bptt(const nmarl_model* m, const nmarl_bwd_args* a, void* stream) {
@@ -1100,18 +1092,16 @@ extern "C" int nmarl_a2c_bptt(const nmarl_model* m, const nmarl_bwd_args* a, voi
   NMARL_CHECK(a->ctx != nullptr, "a2c_bptt: nmarl_bwd_args.ctx is NULL (nmarl_create)");
   cudaStream_t side = a->ctx->side;
   cudaEvent_t ev_fork = a->ctx->fork, ev_join = a->ctx->join;
-  // fused_heads (saved-rollout path): the heads / loss kernel (nmarl_a2c_train_heads) is folded in.  Only the last
-  // HEAD_LEAD time steps are computed on the caller's stream before the reverse chain starts; the remaining steps run
-  // on the side stream beside the first reverse steps (the chain reaches step T-1-HEAD_LEAD long after they are done).
+  // Heads / loss partials / sv_dlv: only the last HEAD_LEAD time steps are computed on the caller's stream before the
+  // reverse chain starts; the remaining steps run on the side stream beside the first reverse steps (the chain reaches
+  // step T-1-HEAD_LEAD long after they are done).
   constexpr int HEAD_LEAD = 6;
-  const int lead = a->fused_heads ? (T < HEAD_LEAD ? T : HEAD_LEAD) : 0;
-  if (a->fused_heads && launch_train_heads(m, a, T - lead, lead, st)) return 1;
+  const int lead = T < HEAD_LEAD ? T : HEAD_LEAD;
+  if (launch_train_heads(m, a, T - lead, lead, st)) return 1;
   NMARL_CUDA(cudaEventRecord(ev_fork, st));
   NMARL_CUDA(cudaStreamWaitEvent(side, ev_fork, 0));
-  if (a->fused_heads) {
-    if (launch_train_heads(m, a, 0, T - lead, side)) return 1;
-    NMARL_CUDA(cudaEventRecord(a->ctx->heads, side));
-  }
+  if (launch_train_heads(m, a, 0, T - lead, side)) return 1;
+  NMARL_CUDA(cudaEventRecord(a->ctx->heads, side));
   {
     HeadK h{};
     h.N = N; h.B = B; h.T = T; h.splits = head_splits((long)B * T); h.n_a = m->n_a; h.fm = a->state_fm;
@@ -1151,7 +1141,7 @@ extern "C" int nmarl_a2c_bptt(const nmarl_model* m, const nmarl_bwd_args* a, voi
     k.ndp = nmarl_tc_ndp(m);
     k.dpT = (use_tc && a->sv_dpT) ? a->sv_dpT + (size_t)t * N * (B / 32) * (2 * k.ndp * 32) : nullptr;
     int rc = 0;
-    if (a->fused_heads && t == T - 1 - lead) NMARL_CUDA(cudaStreamWaitEvent(st, a->ctx->heads, 0));   // dlv of steps < T - lead
+    if (t == T - 1 - lead) NMARL_CUDA(cudaStreamWaitEvent(st, a->ctx->heads, 0));   // dlv of steps < T - lead
     if (a->ev_step) NMARL_CUDA(cudaEventRecord((cudaEvent_t)a->ev_step[2 * t], st));
     if (use_tc) rc = nmarl_tc_launch_bwd(m, k, st);
     else

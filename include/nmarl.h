@@ -163,7 +163,7 @@ typedef struct {
                            /* passes offsets 0..T and then calls nmarl_rng_advance(rng, T + 1). */
                            /* nmarl_cacc_reset draws from the same generator with counter =     */
                            /* episode << 8 | platoon, lane = env and the tag 0x454e5601         */
-  const int32_t* act_in;   /* v-call / train: [N][B] same-step actions                         */
+  const int32_t* act_in;   /* v-call: [N][B] same-step actions                                 */
   float* v;                /* v-call: [N][B]                                                   */
   const float* wpack;      /* packed 3xTF32 operands (nmarl_pack_weights) or NULL.  When set and  */
                            /* B % 128 == 0 and n_h == 64 the wgmma tensor-core kernel is used,  */
@@ -217,7 +217,8 @@ int nmarl_nstep_return_adv(int n_agent, int B, int T, int NR, const double* rewa
  *   (tensor-core path: sv_dz = [T][N][B/32][256] gate-bias partial sums per 32 rows, sv_dpre unused)
  *   dh_rec, dc_rec [2][N][B][64]   dmsg [2][N][MAX_NBR][B][64]
  *   wt [n_wt] transposed weights   ws: split-K workspace of ws_floats floats
- *   loss_part float [T][N][tiles][4] per-CTA partial sums (policy, value, entropy, pad)
+ *   loss_part float [T][N][tiles][4] partial sums (policy, value, entropy, pad) in 64-row tiles; each
+ *             even tile holds the sum of 128 rows and the odd tile after it holds zeros
  *   grads [n_param] (fully overwritten)
  */
 typedef struct {
@@ -252,20 +253,17 @@ typedef struct {
   void** ev_step;            /* optional timing hooks (bench.py): 2*T cudaEvent_t, recorded on `stream` before /
                                 after the cell kernel of reverse step t at [2t], [2t+1]; NULL = none               */
   void** ev_wgrad;           /* optional: 2 cudaEvent_t around the weight-gradient GEMM kernel; NULL = none         */
-  int32_t fused_heads;       /* nmarl_a2c_bptt also does the work of nmarl_a2c_train_heads (do not call it), most of it
-                                on the ctx's side stream beside the first reverse steps                              */
 } nmarl_bwd_args;
 
 int nmarl_loss_tiles(const nmarl_model* m, int B);       /* tiles per agent in loss_part      */
 int64_t nmarl_ws_floats(const nmarl_model* m, int B, int T);   /* required workspace          */
 int nmarl_a2c_backward(const nmarl_model* m, const nmarl_bwd_args* a, void* stream);
-/* the two halves, exposed for tests: training forward (saves activations, loss partials,
- * head gradients) and the reverse pass + weight gradients */
+/* the two halves: the training forward re-runs the T cell steps from states_bw and saves the activations
+ * (sv_xin, sv_sh, sv_gates, sv_enc) and h_seq / c_seq / msg_seq.  nmarl_a2c_bptt computes the heads, the loss
+ * partials and sv_dlv = d(loss)/d(logits, v) from h_seq, then the reverse pass and the weight gradients.
+ * When the rollout p-calls already saved the activations (nmarl_fwd_args.sv_*), call nmarl_a2c_bptt alone. */
 int nmarl_a2c_train_forward(const nmarl_model* m, const nmarl_bwd_args* a, void* stream);
 int nmarl_a2c_bptt(const nmarl_model* m, const nmarl_bwd_args* a, void* stream);
-/* when the rollout p-calls already saved the activations (nmarl_fwd_args.sv_*): only the heads, the loss
- * partials and d(loss)/d(logits, v) are computed from h_seq -- replaces nmarl_a2c_train_forward             */
-int nmarl_a2c_train_heads(const nmarl_model* m, const nmarl_bwd_args* a, void* stream);
 
 /* ---- K10: global-norm clip + TF-semantics RMSProp -------------------------------------------
  * Replaces tf.clip_by_global_norm + tf.train.RMSPropOptimizer (agents/policies.py:34-39,

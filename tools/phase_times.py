@@ -47,8 +47,7 @@ def main():
         ev[2].record()
         a = e._bwd_args(e.T_cur)
         assert getattr(e, 'saved_rollout', False), 'phase map assumes the fused-save rollout'
-        ev[3].record()                      # 'heads' is folded into the BPTT call (side stream) on the product path
-        a.fused_heads = 1
+        ev[3].record()                      # 'heads' is part of the BPTT call (side stream)
         L.check(L.lib().nmarl_a2c_bptt(C.byref(e.model), C.byref(a), L.stream()), 'bptt')
         e.saved_rollout = False
         ev[4].record()
