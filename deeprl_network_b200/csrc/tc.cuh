@@ -130,6 +130,9 @@ __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// wait until at most N committed wgmma groups of this warp are still in flight
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
 
 // D[64 x N] (+)= A[64 rows x 8 tf32, smem desc] * B[N rows x 8 tf32, smem desc]^T, issued by one whole warpgroup.
 // Accumulator fragment (N/2 floats per thread): d[4j + {0,1}] = row 16*warp + lane/4, columns 8j + 2*(lane%4) + {0,1};
@@ -168,6 +171,24 @@ __device__ __forceinline__ void wgmma_tf32(int N, float* d, uint64_t da, uint64_
     case 128: wgmma_tf32_n128(d, da, db, acc); break;
     case 192: wgmma_tf32_n192(d, da, db, acc); break;
     default: wgmma_tf32_n256(d, da, db, acc); break;
+  }
+}
+template <int N>
+__device__ __forceinline__ void wgmma_tf32(float* d, uint64_t da, uint64_t db, uint32_t acc) {
+  static_assert(N == 64 || N == 128 || N == 192 || N == 256, "wgmma tf32 widths used here");
+  if constexpr (N == 64) wgmma_tf32_n64(d, da, db, acc);
+  else if constexpr (N == 128) wgmma_tf32_n128(d, da, db, acc);
+  else if constexpr (N == 192) wgmma_tf32_n192(d, da, db, acc);
+  else wgmma_tf32_n256(d, da, db, acc);
+}
+// the first KS 8-deep k-steps of a 32-deep k-block of a 3xTF32 GEMM of width N, straight-line code
+template <int N, int KS>
+__device__ __forceinline__ void wgmma_kblock_3x(float* d, uint64_t a_hi, uint64_t a_lo, uint64_t b_hi, uint64_t b_lo, bool first) {
+#pragma unroll
+  for (int ks = 0; ks < KS; ++ks) {
+    wgmma_tf32<N>(d, a_hi + 2 * ks, b_hi + 2 * ks, (first && ks == 0) ? 0u : 1u);
+    wgmma_tf32<N>(d, a_hi + 2 * ks, b_lo + 2 * ks, 1u);
+    wgmma_tf32<N>(d, a_lo + 2 * ks, b_hi + 2 * ks, 1u);
   }
 }
 // one 32-deep k-block of a 3xTF32 GEMM: a_hi*b_hi + a_hi*b_lo + a_lo*b_hi per 8-deep k-step

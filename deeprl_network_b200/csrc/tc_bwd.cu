@@ -18,7 +18,6 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_cell_bwd_kernel(const __grid
                                                                     const __grid_constant__ BwdK k) {
   extern __shared__ uint8_t smem_raw[];
   const Smem sm = smem_map(smem_raw);
-  KbEnt* sched = sm.sched;
 
   const int i = blockIdx.y;
   const nmarl_agent& ag = m.agent[i];
@@ -31,17 +30,15 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_cell_bwd_kernel(const __grid
 
   if (tid == 0) {
     init_barriers(sm);
-    int n = 0;
+    SchedBuilder sb(sm);
     // dgrad k-blocks in the order the row threads produce dz: gate o first (its inputs are already in registers from
     // the dc computation), then i and u (which share their two loads), then f
     const int korder[8] = {4, 5, 0, 1, 6, 7, 2, 3};
-    for (int q = 0; q < 8; ++q) sched[n++] = make_kb(ag.tp_gT, SD + NH, NG, korder[q], 0, q == 0, 0, q == 7);
-    if (VAR != NMARL_IA2C && Km > 0)
-      for (int kb = 0; kb < 2; ++kb) sched[n++] = make_kb(ag.tp_mT, Km, NH, kb, 0, kb == 0, 0, kb == 1);
-    *sm.n_kb = n;
+    sb.gemm(ag.tp_gT, SD + NH, NG, 0, DONE_ACC, korder);
+    if (VAR != NMARL_IA2C && Km > 0) sb.gemm(ag.tp_mT, Km, NH, 0, DONE_ACC);   // N = Km: none without neighbours
+    sb.finish();
   }
   __syncthreads();
-  const int n_kb = *sm.n_kb;
   tc::pdl_launch_dependents();       // PDL (tc.cuh): the prologue overlapped the previous reverse step's tail
   tc::pdl_wait();
 
@@ -261,7 +258,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_cell_bwd_kernel(const __grid
       }
     }
   } else {
-    mma_loop(sched, n_kb, sm.bst, sm.ast, sm.b_full, sm.a_full, sm.a_empty, sm.enc_full, sm.acc_full, sm.acc, k.wpack, k.tc_err);
+    mma_loop<0, 64, 128, 192, 256>(sm, k.wpack, k.tc_err);
   }
 }
 

@@ -34,7 +34,6 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_cell_fwd_kernel(const __grid
   static_assert(HW <= EW, "a set's HW partial head sums live in its EW gate-f staging columns");
   extern __shared__ uint8_t smem_raw[];
   const Smem sm = smem_map(smem_raw);
-  KbEnt* sched = sm.sched;
 
   const nmarl_fwd_args& a = k.a;
   const int i = blockIdx.y;
@@ -51,24 +50,19 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_cell_fwd_kernel(const __grid
     // block of the accumulator region, one completion barrier), then the gate GEMM over [s | h^] ----------------
     // An agent without neighbours has zero-width fingerprint / message operands: they get no k-block (and no packed
     // tiles to copy), and the row threads feed relu(0 + b) for them, as the FFMA kernel does.
-    int n = 0;
-    const int KG = SD + NH, nG = KG / 32;
-    sched[n++] = make_kb(ag.tp_x, 64, Kx, 0, ACC_COL, 1, 0, 0);                          // X (Kx <= 32 on this path)
-    if (VAR == NMARL_NC && ag.n_nbr > 0) sched[n++] = make_kb(ag.tp_p, 64, ag.n_nbr * n_a, 0, ACC_COL + 64, 1, 0, 0);
+    SchedBuilder sb(sm);
+    sb.gemm(ag.tp_x, 64, Kx, ACC_COL, DONE_NONE);                                           // X (Kx <= 32 on this path)
+    if (VAR == NMARL_NC) sb.gemm(ag.tp_p, 64, ag.n_nbr * n_a, ACC_COL + 64, DONE_NONE);     // no neighbours: K = 0
     if (VAR != NMARL_IA2C) {
-      const int nM = (VAR == NMARL_IC3) ? 2 : 2 * ag.n_nbr;
       const int KM = (VAR == NMARL_IC3) ? NH : NH * ag.n_nbr;
-      const int mcol = (VAR == NMARL_NC) ? ACC_COL + 128 : ACC_COL + 64;
-      for (int j = 0; j < nM; ++j) sched[n++] = make_kb(ag.tp_m, 64, KM, j, mcol, j == 0, 0, 0);
+      sb.gemm(ag.tp_m, 64, KM, (VAR == NMARL_NC) ? ACC_COL + 128 : ACC_COL + 64, DONE_NONE);
     }
-    sched[n - 1].last_enc = 1;                          // the last encoder GEMM actually scheduled completes enc_full
-    for (int g = 0; g < nG; ++g) sched[n++] = make_kb(ag.tp_g, 256, KG, g, ACC_COL, g == 0, 0, g == nG - 1);
-    if (VAR == NMARL_DIAL && MODE != MODE_V)
-      for (int j = 0; j < 2; ++j) sched[n++] = make_kb(ag.tp_mfc, 64, NH, j, ACC_COL, j == 0, j == 1, 0);
-    *sm.n_kb = n;
+    sm.seg[sb.ns - 1].done = DONE_ENC;                  // the last encoder GEMM actually scheduled completes enc_full
+    sb.gemm(ag.tp_g, 256, SD + NH, ACC_COL, DONE_ACC);
+    if (VAR == NMARL_DIAL && MODE != MODE_V) sb.gemm(ag.tp_mfc, 64, NH, ACC_COL, DONE_ENC);
+    sb.finish();
   }
   __syncthreads();
-  const int n_kb = *sm.n_kb;
   // PDL: the prologue above overlapped the tail of the previous kernel of the stream; from here on the kernel reads
   // what that kernel (env step / previous cell call) wrote.
   tc::pdl_launch_dependents();
@@ -323,10 +317,12 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_cell_fwd_kernel(const __grid
             logit[2] = fmaf(hn[x], w4.z, logit[2]); logit[3] = fmaf(hn[x], w4.w, logit[3]);
           }
         } else {
+          // one logit at a time (each still sums its 8 units in order): with the units outer, ptxas hoisted all
+          // HW x 8 weight loads and the HW = 16 saving instantiations spilled
 #pragma unroll
-          for (int x = 0; x < 8; ++x)
+          for (int cc = 0; cc < HW; ++cc)
 #pragma unroll
-            for (int cc = 0; cc < HW; ++cc)
+            for (int x = 0; x < 8; ++x)
               if (cc < n_a) logit[cc] = fmaf(hn[x], __ldg(P + ag.o_pi_w + (u0 + x) * n_a + cc), logit[cc]);
         }
       }
@@ -426,7 +422,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_cell_fwd_kernel(const __grid
     if (prof) prof[31] = pi_;
   } else {
     // =================================== MMA warpgroup ===================================================
-    mma_loop(sched, n_kb, sm.bst, sm.ast, sm.b_full, sm.a_full, sm.a_empty, sm.enc_full, sm.acc_full, sm.acc, a.wpack, a.tc_err);
+    mma_loop<MMA_PIPE | MMA_PARTIAL, 64, 256>(sm, a.wpack, a.tc_err);
   }
   __syncthreads();
 }

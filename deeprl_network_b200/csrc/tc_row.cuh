@@ -36,10 +36,15 @@ __device__ __forceinline__ uint32_t acc_idx(uint32_t row, uint32_t col) {
   return row * ACC_COLS + (col & ~31u) + ((((col >> 2) ^ row) & 7u) << 2) + (col & 3u);
 }
 
-struct KbEnt {
-  uint32_t off_bytes, bytes;
-  uint16_t dcol;                                          // accumulator column of this GEMM
-  uint8_t ksteps, first, last_enc, last_acc, pad0, pad1;
+constexpr int MAX_SEG = 8;
+// The k-block schedule: a flat list of streamed weight k-blocks (thread 0 of the MMA warpgroup copies them in this
+// order) and the GEMMs ("segments") it is made of.  A segment's width N is uniform over the CTA, so the MMA warpgroup
+// dispatches on it once per GEMM and runs straight-line wgmma code of that width.
+struct KbEnt { uint32_t off_bytes, bytes; };              // one [hi | lo] weight k-block in the packed operands
+enum : uint8_t { DONE_NONE = 0, DONE_ENC, DONE_ACC };     // completion barrier a GEMM arrives on once stored
+struct Seg {
+  uint16_t n, dcol;                                       // GEMM width N, accumulator column of the result
+  uint8_t kb0, nkb, ks_last, done;                        // k-blocks [kb0, kb0 + nkb), k-steps of the last one
 };
 
 struct RowCtx {
@@ -182,77 +187,139 @@ __device__ __forceinline__ void row_barrier() { asm volatile("bar.sync 1, %0;" :
 __device__ __forceinline__ void mma_wg_sync() { asm volatile("bar.sync 2, 128;" ::: "memory"); }
 
 
-// ---- the MMA warpgroup ------------------------------------------------------------------------------------------
-// All 128 threads: per k-block the 3xTF32 wgmma chain into the register accumulator; a finished GEMM (the next entry
-// starts a new one, or a completion flag is set) is stored into the staging area at its column dcol.  Thread 0 also
-// streams the weight k-blocks: one cp.async.bulk (TMA engine) per k-block into the S_STAGES ring, refilled as soon as
-// the warpgroup has retired the MMAs that read a stage.  a_empty / enc_full / acc_full count one arrival per thread.
-__device__ __forceinline__ void mma_loop(const KbEnt* sched, int n_kb, uint8_t* bst, uint8_t* ast, uint64_t* b_full,
-                                         uint64_t* a_full, uint64_t* a_empty, uint64_t* enc_full, uint64_t* acc_full,
-                                         float* acc_s, const float* wpack, int* err) {
-  const int t = threadIdx.x - MMA_WARP0 * 32, w = t >> 5, l = t & 31;
-  const uint8_t* wp = reinterpret_cast<const uint8_t*>(wpack);
-  auto fetch = [&](int q) {
-    const int st = q % S_STAGES;
-    const KbEnt e = sched[q];
-    tc::mbar_arrive_expect_tx(&b_full[st], e.bytes);
-    tc::bulk_g2s(bst + st * STAGE_BYTES, wp + e.off_bytes, e.bytes, &b_full[st]);
-  };
-  if (t == 0)
-    for (int q = 0; q < S_STAGES && q < n_kb; ++q) fetch(q);
-  float d[128];
-#pragma unroll
-  for (int j = 0; j < 128; ++j) d[j] = 0.f;
-  for (int q = 0; q < n_kb; ++q) {
-    const int st = q % S_STAGES, slot = q & (A_SLOTS - 1);
-    const KbEnt e = sched[q];
-    tc::mbar_wait(&b_full[st], (q / S_STAGES) & 1, err, 31);
-    tc::mbar_wait(&a_full[slot], (q / A_SLOTS) & 1, err, 32);
-    const int N = (int)(e.bytes / 256);
-    uint8_t* b = bst + st * STAGE_BYTES;
-    uint8_t* a = ast + slot * A_SLOT_BYTES;
-    tc::wgmma_fence();
-    tc::wgmma_kblock_3x(N, d, tc::smem_desc_sw128(a), tc::smem_desc_sw128(a + A_TILE), tc::smem_desc_sw128(b),
-                        tc::smem_desc_sw128(b + N * 128), e.ksteps, e.first != 0);
-    tc::wgmma_commit();
-    tc::wgmma_wait_all();
-    tc::mbar_arrive(&a_empty[slot]);
-    mma_wg_sync();                                         // every thread has retired the k-block: stage st is free
-    if (t == 0 && q + S_STAGES < n_kb) fetch(q + S_STAGES);
-    if (e.last_enc || e.last_acc || q + 1 == n_kb || sched[q + 1].first) {
-      const uint32_t r0 = 16 * w + (l >> 2);
-#pragma unroll
-      for (int j = 0; j < 32; ++j) {
-        if (8 * j < N) {
-          const uint32_t col = e.dcol + 8 * j + 2 * (l & 3);
-#pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            const uint32_t r = r0 + 8 * h;
-            *reinterpret_cast<float2*>(acc_s + acc_idx(r, col)) = make_float2(d[4 * j + 2 * h], d[4 * j + 2 * h + 1]);
-          }
-        }
-      }
-      if (e.last_enc) tc::mbar_arrive(enc_full);
-      if (e.last_acc) tc::mbar_arrive(acc_full);
-    }
-  }
-}
-__device__ __forceinline__ KbEnt make_kb(int off_floats, int N, int K, int kb, int dcol, int first, int last_enc, int last_acc) {
-  KbEnt e;
-  e.off_bytes = (uint32_t)(off_floats + kb * 2 * N * 32) * 4u;
-  e.bytes = 2u * N * 128u;
-  const int k8 = (K + 7) / 8 * 8;
-  e.ksteps = (uint8_t)min(4, (k8 - kb * 32) / 8);
-  e.dcol = (uint16_t)dcol; e.first = first; e.last_enc = last_enc; e.last_acc = last_acc;
-  e.pad0 = e.pad1 = 0;
-  return e;
-}
 // [B stages | A slots | accumulator staging | mbarriers | schedule], 1024-byte aligned tiles
 struct Smem {
   uint8_t* bst; uint8_t* ast; float* acc;
   uint64_t *b_full, *a_full, *a_empty, *enc_full, *acc_full;
-  int* n_kb; KbEnt* sched;
+  int* n_kb; int* n_seg; KbEnt* sched; Seg* seg;
 };
+
+// Schedule builder (thread 0, before the roles start).  gemm() appends one GEMM D[64 x N] = A[64 x K] W[K x N] of
+// the packed operand at float offset off: its ceil(K / 32) k-blocks in k order, or in the order `order` lists them.
+// Only the last k-block may be partial, and only at N = 64 (K of the observation / fingerprint encoders); a GEMM
+// without k-blocks (K = 0) adds nothing.
+struct SchedBuilder {
+  const Smem& s;
+  int nk, ns;
+  __device__ __forceinline__ explicit SchedBuilder(const Smem& sm) : s(sm), nk(0), ns(0) {}
+  __device__ __forceinline__ void gemm(int off_floats, int N, int K, int dcol, uint8_t done, const int* order = nullptr) {
+    const int nkb = (K + 31) / 32;
+    if (nkb == 0) return;
+    int kb = 0;
+    for (int j = 0; j < nkb; ++j) {
+      kb = order ? order[j] : j;
+      s.sched[nk + j] = KbEnt{(uint32_t)(off_floats + kb * 2 * N * 32) * 4u, 2u * N * 128u};
+    }
+    const int k8 = (K + 7) / 8 * 8;
+    s.seg[ns++] = Seg{(uint16_t)N, (uint16_t)dcol, (uint8_t)nk, (uint8_t)nkb, (uint8_t)min(4, (k8 - kb * 32) / 8), done};
+    nk += nkb;
+  }
+  __device__ __forceinline__ void finish() { *s.n_kb = nk; *s.n_seg = ns; }
+};
+
+// ---- the MMA warpgroup ------------------------------------------------------------------------------------------
+// All 128 threads run the GEMMs of the schedule in order; per 8-deep k-step the 3xTF32 wgmma chain hi*hi, hi*lo,
+// lo*hi into the register accumulator.  Thread 0 also streams the weight k-blocks: one cp.async.bulk (TMA engine) per
+// k-block into the S_STAGES ring.  One k-block of MMAs stays in flight: k-block q is issued before the warpgroup waits
+// for q - 1 (wgmma.wait_group 1), and only then are q - 1's A slot (a_empty) and B stage (refilled with k-block
+// q - 1 + S_STAGES) released.  At the end of a GEMM everything is retired, its last k-block released, and the result
+// stored into the staging area at column dcol; then it arrives on its completion barrier.  a_empty / enc_full /
+// acc_full count one arrival per thread.
+struct MmaCtx {
+  const Smem& s;
+  const uint8_t* wp;
+  int* err;
+  int t, n_kb;
+  __device__ __forceinline__ void fetch(int q) const {
+    const int st = q % S_STAGES;
+    const KbEnt e = s.sched[q];
+    tc::mbar_arrive_expect_tx(&s.b_full[st], e.bytes);
+    tc::bulk_g2s(s.bst + st * STAGE_BYTES, wp + e.off_bytes, e.bytes, &s.b_full[st]);
+  }
+  // k-block q has retired in every thread of the warpgroup: free its A slot and refill its B stage
+  __device__ __forceinline__ void release(int q) const {
+    tc::mbar_arrive(&s.a_empty[q & (A_SLOTS - 1)]);
+    mma_wg_sync();
+    if (t == 0 && q + S_STAGES < n_kb) fetch(q + S_STAGES);
+  }
+  // wait for k-block q's operands and issue its KS k-steps (one commit group)
+  template <int N, int KS>
+  __device__ __forceinline__ void issue(float* d, int q, bool first) const {
+    const int st = q % S_STAGES, slot = q & (A_SLOTS - 1);
+    tc::mbar_wait(&s.b_full[st], (q / S_STAGES) & 1, err, 31);
+    tc::mbar_wait(&s.a_full[slot], (q / A_SLOTS) & 1, err, 32);
+    const uint8_t* b = s.bst + st * STAGE_BYTES;
+    const uint8_t* a = s.ast + slot * A_SLOT_BYTES;
+    tc::wgmma_fence();
+    tc::wgmma_kblock_3x<N, KS>(d, tc::smem_desc_sw128(a), tc::smem_desc_sw128(a + A_TILE), tc::smem_desc_sw128(b),
+                               tc::smem_desc_sw128(b + N * 128), first);
+    tc::wgmma_commit();
+  }
+};
+
+// MMA loop options.  MMA_PIPE: keep one k-block in flight (above); without it every k-block is retired and released
+// before the next is issued.  MMA_PARTIAL: the schedule has GEMMs whose last k-block is partial (the forward's
+// observation / fingerprint encoders, N = 64); without it only whole k-blocks are compiled.
+enum : int { MMA_PIPE = 1, MMA_PARTIAL = 2 };
+
+template <int OPT, int N, int KS_LAST>
+__device__ __forceinline__ void gemm_segment(const MmaCtx& x, const Seg& sg) {
+  float d[N / 2];
+#pragma unroll
+  for (int j = 0; j < N / 2; ++j) d[j] = 0.f;
+  const int q0 = sg.kb0, qe = q0 + sg.nkb - 1;             // qe: the (possibly partial) last k-block
+  constexpr bool PIPE = (OPT & MMA_PIPE) != 0;
+  for (int q = q0; q < qe; ++q) {
+    x.issue<N, 4>(d, q, q == q0);
+    if (!PIPE) { tc::wgmma_wait<0>(); x.release(q); }
+    else if (q > q0) { tc::wgmma_wait<1>(); x.release(q - 1); }
+  }
+  x.issue<N, KS_LAST>(d, qe, qe == q0);
+  tc::wgmma_wait<0>();
+  if (PIPE && qe > q0) x.release(qe - 1);
+  x.release(qe);
+  const int w = x.t >> 5, l = x.t & 31;
+  const uint32_t r0 = 16 * w + (l >> 2);
+#pragma unroll
+  for (int j = 0; j < N / 8; ++j) {
+    const uint32_t col = sg.dcol + 8 * j + 2 * (l & 3);
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+      *reinterpret_cast<float2*>(x.s.acc + acc_idx(r0 + 8 * h, col)) = make_float2(d[4 * j + 2 * h], d[4 * j + 2 * h + 1]);
+  }
+}
+// A partial last k-block occurs only in the N = 64 encoder GEMMs of the observations and fingerprints (K <= 32), so
+// only N = 64 (with MMA_PARTIAL) has the shorter variants; false: the segment is not one this kernel can run.
+template <int OPT, int N>
+__device__ __forceinline__ bool gemm_segment_n(const MmaCtx& x, const Seg& sg) {
+  if (sg.n != N) return false;
+  if constexpr (N == 64 && (OPT & MMA_PARTIAL) != 0) {
+    switch (sg.ks_last) {
+      case 1: gemm_segment<OPT, N, 1>(x, sg); return true;
+      case 2: gemm_segment<OPT, N, 2>(x, sg); return true;
+      case 3: gemm_segment<OPT, N, 3>(x, sg); return true;
+    }
+  }
+  if (sg.ks_last != 4) return false;
+  gemm_segment<OPT, N, 4>(x, sg);
+  return true;
+}
+// NS: the GEMM widths the kernel's schedule uses.  A segment no instantiation runs is a schedule bug: the warpgroup
+// stops and reports tc_err 30 (the row threads' waits then time out instead of hanging).
+template <int OPT, int... NS>
+__device__ __forceinline__ void mma_loop(const Smem& s, const float* wpack, int* err) {
+  const MmaCtx x{s, reinterpret_cast<const uint8_t*>(wpack), err, (int)threadIdx.x - MMA_WARP0 * 32, *s.n_kb};
+  if (x.t == 0)
+    for (int q = 0; q < S_STAGES && q < x.n_kb; ++q) x.fetch(q);
+  const int n_seg = *s.n_seg;
+  for (int i = 0; i < n_seg; ++i) {
+    const Seg sg = s.seg[i];
+    const bool known = (gemm_segment_n<OPT, NS>(x, sg) || ...);
+    if (!known) { if (x.t == 0) atomicCAS(err, 0, 30); break; }
+    if (sg.done == DONE_ENC) tc::mbar_arrive(s.enc_full);
+    if (sg.done == DONE_ACC) tc::mbar_arrive(s.acc_full);
+  }
+}
 __device__ __forceinline__ Smem smem_map(uint8_t* raw) {
   uint8_t* s = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(raw) + 1023) & ~uintptr_t(1023));
   Smem m;
@@ -263,7 +330,9 @@ __device__ __forceinline__ Smem smem_map(uint8_t* raw) {
   m.b_full = bars; m.a_full = bars + S_STAGES; m.a_empty = m.a_full + A_SLOTS;
   m.enc_full = m.a_empty + A_SLOTS; m.acc_full = m.enc_full + 1;
   m.n_kb = reinterpret_cast<int*>(m.acc_full + 1);
+  m.n_seg = m.n_kb + 1;
   m.sched = reinterpret_cast<KbEnt*>(m.n_kb + 2);
+  m.seg = reinterpret_cast<Seg*>(m.sched + MAX_KB);
   return m;
 }
 __device__ __forceinline__ void init_barriers(const Smem& s) {
@@ -274,7 +343,7 @@ __device__ __forceinline__ void init_barriers(const Smem& s) {
   tc::fence_barrier_init();
 }
 constexpr size_t TC_SMEM = 1024 /*align slack*/ + S_STAGES * STAGE_BYTES + A_SLOTS * A_SLOT_BYTES + ACC_BYTES + 16 * 8 /*mbarriers*/ +
-                           8 + MAX_KB * sizeof(KbEnt);
+                           8 + MAX_KB * sizeof(KbEnt) + MAX_SEG * sizeof(Seg);
 static_assert(TC_SMEM <= 232448, "cell kernels exceed the 227 KB of dynamic shared memory");
 
 }  // namespace tcrow
