@@ -189,7 +189,8 @@ class OracleCACC:
                 v0 = np.ones(n) * self.v_star * (1.5 + (np.random.rand() if u01 is None else u01))
             self.v0s = np.ones(self.T + 1) * self.v_star
             dec = np.linspace(v0[0], self.v_star, 300)
-            self.v0s[:len(dec)] = dec
+            # episodes shorter than the 300-step ramp keep its first T + 1 entries (the reference needs T >= 299)
+            self.v0s[:len(dec)] = dec[:self.T + 1]
         self.collision = False
         self.hs_cur, self.vs_cur, self.us_cur = h0, v0, np.zeros(n)
         self.fp = np.ones((n, self.n_a)) / self.n_a
