@@ -76,14 +76,14 @@ class BwdArgs(C.Structure):
                 ('wt', C.c_void_p), ('ws', C.c_void_p), ('ws_floats', C.c_int64),
                 ('loss_part', C.c_void_p), ('grads', C.c_void_p), ('wpack', C.c_void_p), ('tc_err', C.c_void_p),
                 ('sv_dzT', C.c_void_p), ('sv_dpT', C.c_void_p), ('state_fm', C.c_int32),
-                ('ctx', C.c_void_p), ('raw_tiles', C.c_int32), ('ev_step', C.c_void_p), ('ev_wgrad', C.c_void_p)]
+                ('ctx', C.c_void_p), ('ev_step', C.c_void_p), ('ev_wgrad', C.c_void_p)]
 
 
 _lib = None
 
 EXPORTS = ['nmarl_last_error', 'nmarl_version', 'nmarl_create', 'nmarl_destroy', 'nmarl_sizeof_bwd_args', 'nmarl_sizeof_fwd_args', 'nmarl_sizeof_model', 'nmarl_sizeof_agent', 'nmarl_sizeof_cacc_cfg',
            'nmarl_cacc_reset', 'nmarl_cacc_step', 'nmarl_pack_weights', 'nmarl_policy_step_p', 'nmarl_policy_step_v', 'nmarl_dial_msg',
-           'nmarl_rng_advance', 'nmarl_nstep_return_adv', 'nmarl_loss_tiles', 'nmarl_ws_floats',
+           'nmarl_rng_advance', 'nmarl_nstep_return_adv', 'nmarl_loss_tiles', 'nmarl_ws_floats', 'nmarl_operand_tile_offset',
            'nmarl_a2c_backward', 'nmarl_a2c_train_forward', 'nmarl_a2c_bptt',
            'nmarl_clip_rmsprop_step', 'nmarl_consensus_update', 'nmarl_eval_record']
 
@@ -112,6 +112,8 @@ def lib():
     L.nmarl_nstep_return_adv.argtypes = [I, I, I, I, P, P, P, P, I, D, D, D, D, P, P, I, P, P, P]
     L.nmarl_loss_tiles.argtypes = [C.POINTER(Model), I]
     L.nmarl_ws_floats.argtypes = [C.POINTER(Model), I, I]
+    L.nmarl_operand_tile_offset.restype = C.c_int64
+    L.nmarl_operand_tile_offset.argtypes = [I, I, I, I, I, I]
     for fn in ('nmarl_a2c_backward', 'nmarl_a2c_train_forward', 'nmarl_a2c_bptt'):
         getattr(L, fn).argtypes = [C.POINTER(Model), C.POINTER(BwdArgs), P]
     L.nmarl_clip_rmsprop_step.argtypes = [C.POINTER(Model), P, P, P, P, F, F, F, P, P, P]

@@ -25,6 +25,13 @@ def tc_eligible(layout, n_env):
     return int(n_env) % 128 == 0 and layout.kx_pad <= 32 and layout.kp_pad <= 32 and layout.n_h == L.NH
 
 
+def operand_tile_shapes(variant, N, B, T, n_h):
+    """sv_dzT, sv_dpT of the tensor-core path (variant: kernel family): one raw fp32 tile of 4 n_h (dz) or ndp (encoder
+    pre-activation gradients) rows x 32 envs per step, agent and 32-env block, indexed by nmarl_operand_tile_offset."""
+    ndp = {'ma2c_nc': 3 * n_h, 'ia2c': n_h}.get(variant, 2 * n_h)
+    return (T, N, B // 32, 4 * n_h * 32), (T, N, B // 32, ndp * 32)
+
+
 class PolicyEngine:
     def __init__(self, layout, n_env, n_step, hp, flat_params=None, device=None, rng_seed=0,
                  distance_mask=None, coop_gamma=-1.0, group=None, use_tc=None, shared_params=None):
@@ -63,7 +70,7 @@ class PolicyEngine:
         self.tc_err = torch.zeros(1, dtype=torch.int32, device=dev)
         # tensor-core path: LSTM state (and its gradients) feature-major [N,64,B] so that lane == env accesses are
         # coalesced; DIAL keeps env-major state (its message kernels are env-major)
-        self.state_fm = self.use_tc and self.variant != 'ma2c_dial' and os.environ.get('NMARL_NO_STATE_FM', '0') != '1'
+        self.state_fm = self.use_tc and self.variant != 'ma2c_dial'
         NH = self.n_h
         self._sshape = (N, NH, B) if self.state_fm else (N, B, NH)
         self.c = [torch.zeros(*self._sshape, **f32) for _ in range(2)]
@@ -108,8 +115,7 @@ class PolicyEngine:
         self.kernel_events = None          # bench.py: list collecting (start, end) CUDA events around each rollout p-call
         self.T_cur = T
         self.launches = 0
-        # single-copy operand tiles for the weight-gradient GEMMs (nmarl_bwd_args.raw_tiles)
-        self.raw_tiles = self.use_tc and os.environ.get('NMARL_RAW_TILES', '1') != '0'
+        self.raw_tiles = self.use_tc           # bench.py reads it: the tensor-core path stores raw operand tiles
         self.bwd_events = None             # bench.py: (step events [2T], wgrad events [2]) recorded inside nmarl_a2c_bptt
         self._ctx = C.c_void_p()
         L.check(L.lib().nmarl_create(C.byref(self._ctx)), 'nmarl_create')
@@ -353,10 +359,10 @@ class PolicyEngine:
         # tensor-core path: sv_dz holds per-tile gate-bias partial sums, sv_dpre is unused (operand tiles instead)
         self.sv_dz = z(T, N, B // 32, 4 * NH) if self.use_tc else z(T, N, B, 4 * NH)
         self.sv_dpre = z(4) if self.use_tc else z(T, N, B, 3 * NH)
-        # tensor-core path: dz / encoder pre-activation gradients additionally as K-major [hi | lo] operand tiles
-        ndp = {'ma2c_nc': 3 * NH, 'ia2c': NH}.get(self.variant, 2 * NH)
-        self.sv_dzT = z(T, N, B // 32, 2 * 4 * NH * 32) if self.use_tc else None
-        self.sv_dpT = z(T, N, B // 32, 2 * ndp * 32) if self.use_tc else None
+        # tensor-core path: dz / encoder pre-activation gradients additionally as K-major raw operand tiles
+        dzT, dpT = operand_tile_shapes(self.variant, N, B, T, NH)
+        self.sv_dzT = z(*dzT) if self.use_tc else None
+        self.sv_dpT = z(*dpT) if self.use_tc else None
         self.sv_dmp = z(T, N, B, NH) if self.variant == 'ma2c_dial' else None
         self.dh_rec, self.dc_rec = z(2, *self._sshape), z(2, *self._sshape)
         self.dmsg = z(2, N, L.MAX_NBR, *self._sshape[1:]) if self.variant != 'ia2c' else None
@@ -383,7 +389,7 @@ class PolicyEngine:
         a.wpack, a.tc_err = L.ptr(self.wpack), L.ptr(self.tc_err)
         a.sv_dzT, a.sv_dpT = L.ptr(self.sv_dzT), L.ptr(self.sv_dpT)
         a.state_fm = int(self.state_fm)
-        a.ctx, a.raw_tiles = self._ctx, int(self.raw_tiles)
+        a.ctx = self._ctx
         if self.bwd_events is not None:
             step_ev, wg_ev = self.bwd_events
             self._ev_arrays = ((C.c_void_p * len(step_ev))(*[ev.cuda_event for ev in step_ev]),

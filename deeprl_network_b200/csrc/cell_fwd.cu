@@ -454,7 +454,7 @@ extern "C" int nmarl_policy_step_p(const nmarl_model* m, const nmarl_fwd_args* a
   NMARL_CHECK(m->variant != NMARL_DIAL || (a->msg_in && a->msg_out), "policy_step_p: DIAL needs msg_in/msg_out");
   NMARL_CHECK(a->sample_mode != NMARL_SAMPLE_UNIFORM || a->uniforms, "policy_step_p: uniforms required");
   NMARL_CHECK(a->sample_mode != NMARL_SAMPLE_PHILOX || a->rng, "policy_step_p: rng state required");
-  NMARL_CHECK(!a->state_fm || nmarl_tc_fwd_supported(m, a), "policy_step_p: feature-major state needs the tensor-core path");
+  NMARL_CHECK(a->state_fm == nmarl_state_fm(m, nmarl_tc_fwd_supported(m, a)), "policy_step_p: " NMARL_STATE_FM_RULE, a->state_fm);
   if (a->sv_sh != nullptr) {                 // rollout p-call that also saves activations for BPTT
     NMARL_CHECK(nmarl_tc_fwd_supported(m, a), "policy_step_p: activation saving needs the tensor-core path (B %% 128 == 0, wpack)");
     NMARL_CHECK(a->sv_xin && a->sv_gates, "policy_step_p: sv_xin / sv_gates missing");
@@ -472,7 +472,7 @@ extern "C" int nmarl_policy_step_v(const nmarl_model* m, const nmarl_fwd_args* a
               "policy_step_v: missing buffers");
   NMARL_CHECK((m->variant != NMARL_NC && m->variant != NMARL_DIAL) || a->fp, "policy_step_v: fp required");
   NMARL_CHECK(m->variant != NMARL_DIAL || a->msg_in, "policy_step_v: DIAL needs msg_in");
-  NMARL_CHECK(!a->state_fm || nmarl_tc_fwd_supported(m, a), "policy_step_v: feature-major state needs the tensor-core path");
+  NMARL_CHECK(a->state_fm == nmarl_state_fm(m, nmarl_tc_fwd_supported(m, a)), "policy_step_v: " NMARL_STATE_FM_RULE, a->state_fm);
   FwdK k{};
   k.a = *a;
   return dispatch_fwd<MODE_V>(m, k, (cudaStream_t)stream);

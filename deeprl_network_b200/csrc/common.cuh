@@ -23,6 +23,11 @@ __host__ __device__ constexpr int nmarl_log2(int x) { return x <= 1 ? 0 : 1 + nm
 
 void nmarl_set_error(const char* fmt, ...);
 
+// The LSTM state layout a call must declare in nmarl_fwd_args / nmarl_bwd_args.state_fm: feature-major on the
+// tensor-core path except for DIAL (its message kernels are env-major), env-major on the FFMA path.
+inline int nmarl_state_fm(const nmarl_model* m, bool tc_path) { return tc_path && m->variant != NMARL_DIAL; }
+#define NMARL_STATE_FM_RULE "state_fm must be 1 on the tensor-core path except for DIAL, else 0 (got %d)"
+
 #define NMARL_CHECK(cond, ...)                         \
   do {                                                 \
     if (!(cond)) {                                     \

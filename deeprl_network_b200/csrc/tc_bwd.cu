@@ -10,12 +10,13 @@
 namespace {
 using namespace tcrow;
 
-// RAW (the default; nmarl_bwd_args.raw_tiles): the operand tiles for the weight-gradient GEMMs are stored once as raw
-// fp32 instead of as a [hi | lo] pair; the weight-gradient kernel splits them in shared memory with the same
-// tc::split_tf32, so both forms feed its MMAs identical operands.
-template <int VAR, bool FM, bool RAW, int HW>
+// The operand tiles for the weight-gradient GEMMs (dz^T, dpre^T) are stored once as raw fp32 (nmarl_tc_tile_offset);
+// the weight-gradient kernel splits them into [hi | lo] in shared memory.
+// State (c, dh, dc, dmsg) is feature-major except for DIAL, whose message kernels are env-major.
+template <int VAR, int HW>
 __global__ void __launch_bounds__(TC_THREADS, 1) tc_cell_bwd_kernel(const __grid_constant__ nmarl_model m,
                                                                     const __grid_constant__ BwdK k) {
+  constexpr bool FM = VAR != NMARL_DIAL;
   extern __shared__ uint8_t smem_raw[];
   const Smem sm = smem_map(smem_raw);
 
@@ -132,19 +133,12 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_cell_bwd_kernel(const __grid
         const int col = (((lane >> 4) & 1) << 3) | (((lane >> 3) & 1) << 2) | (((lane >> 2) & 1) << 1) | ((lane >> 1) & 1);
         if ((lane & 1) == 0) k.sv_dz[((size_t)i * (B / 32) + (b0 / 32) + rh) * NG + g * NH + e0 + col] = a[0];
       }
-      if (k.dzT != nullptr) {                 // dz^T tile for the tensor-core wgrad: K-major over rows, hi | lo
-        uint8_t* tile = reinterpret_cast<uint8_t*>(k.dzT) + ((size_t)i * (B / 32) + (b0 / 32) + rh) * (size_t)((RAW ? 1 : 2) * 256 * 128);
+      if (k.dzT != nullptr) {                 // dz^T tile for the tensor-core wgrad: K-major over rows
+        uint8_t* tile = reinterpret_cast<uint8_t*>(k.dzT + nmarl_tc_tile_offset(NG, 0, m.n_agent, B / 32, i, b0 / 32 + rh));
 #pragma unroll
         for (int j = 0; j < EW; ++j) {
           const uint32_t off = tc::sw128_offset((uint32_t)(g * NH + e0 + j), (uint32_t)lane);
-          if constexpr (RAW) {
-            __stcs(reinterpret_cast<float*>(tile + off), dz[j]);
-          } else {
-            float hi, lo;
-            tc::split_tf32(dz[j], hi, lo);
-            __stcs(reinterpret_cast<float*>(tile + off), hi);                       // read once, by the wgrad kernel
-            __stcs(reinterpret_cast<float*>(tile + 256 * 128 + off), lo);
-          }
+          __stcs(reinterpret_cast<float*>(tile + off), dz[j]);                      // read once, by the wgrad kernel
         }
       }
       produce_act(c, dz);                      // the gate's two k-blocks of the 256-deep dgrad contraction
@@ -180,20 +174,13 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_cell_bwd_kernel(const __grid
 #pragma unroll
     for (int j = 0; j < EW; ++j) dpm[j] = 0.f;
     uint8_t* dptile = (k.dpT != nullptr)
-        ? reinterpret_cast<uint8_t*>(k.dpT) + ((size_t)i * (B / 32) + (b0 / 32) + rh) * (size_t)((RAW ? 1 : 2) * k.ndp * 128) : nullptr;
+        ? reinterpret_cast<uint8_t*>(k.dpT + nmarl_tc_tile_offset(k.ndp, 0, m.n_agent, B / 32, i, b0 / 32 + rh)) : nullptr;
     auto put_dp = [&](int n0, const float (&vals)[EW]) {        // encoder pre-activation grads as K-major tiles
       if (dptile == nullptr) return;
 #pragma unroll
       for (int j = 0; j < EW; ++j) {
         const uint32_t off = tc::sw128_offset((uint32_t)(n0 + j), (uint32_t)lane);
-        if constexpr (RAW) {
-          __stcs(reinterpret_cast<float*>(dptile + off), vals[j]);
-        } else {
-          float hi, lo;
-          tc::split_tf32(vals[j], hi, lo);
-          __stcs(reinterpret_cast<float*>(dptile + off), hi);
-          __stcs(reinterpret_cast<float*>(dptile + (size_t)k.ndp * 128 + off), lo);
-        }
+        __stcs(reinterpret_cast<float*>(dptile + off), vals[j]);
       }
     };
 #pragma unroll
@@ -264,9 +251,9 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_cell_bwd_kernel(const __grid
 
 NMARL_PARAMS_FIT(nmarl_model, BwdK);                                             // tc_cell_bwd_kernel
 
-template <int VAR, bool FM, bool RAW, int HW>
-int launch_tc_bwd_fm(const nmarl_model* m, const BwdK& k, cudaStream_t st) {
-  auto kern = tc_cell_bwd_kernel<VAR, FM, RAW, HW>;
+template <int VAR, int HW>
+int launch_tc_bwd_hw(const nmarl_model* m, const BwdK& k, cudaStream_t st) {
+  auto kern = tc_cell_bwd_kernel<VAR, HW>;
   static bool configured = false;
   if (!configured) {
     NMARL_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TC_SMEM));
@@ -276,12 +263,6 @@ int launch_tc_bwd_fm(const nmarl_model* m, const BwdK& k, cudaStream_t st) {
   NMARL_CUDA(nmarl_launch(kern, grid, dim3(TC_THREADS), TC_SMEM, st, true, *m, k));
   NMARL_LAUNCH_CHECK();
   return 0;
-}
-
-template <int VAR, int HW>
-int launch_tc_bwd_hw(const nmarl_model* m, const BwdK& k, cudaStream_t st) {
-  if (k.raw_tiles) return k.state_fm ? launch_tc_bwd_fm<VAR, true, true, HW>(m, k, st) : launch_tc_bwd_fm<VAR, false, true, HW>(m, k, st);
-  return k.state_fm ? launch_tc_bwd_fm<VAR, true, false, HW>(m, k, st) : launch_tc_bwd_fm<VAR, false, false, HW>(m, k, st);
 }
 
 template <int VAR>

@@ -26,9 +26,10 @@ namespace {
 
 using namespace tcrow;
 
-template <int VAR, int MODE, bool FM, int HW>
+template <int VAR, int MODE, int HW>
 __global__ void __launch_bounds__(TC_THREADS, 1) tc_cell_fwd_kernel(const __grid_constant__ nmarl_model m,
                                                                     const __grid_constant__ FwdK k) {
+  constexpr bool FM = VAR != NMARL_DIAL;                           // state layout: DIAL's message kernels are env-major
   constexpr bool SAVE = (MODE == MODE_PS);                         // store activations for BPTT
   constexpr bool SAMPLE = (MODE == MODE_P || MODE == MODE_PS);     // p-call: sample actions
   static_assert(HW <= EW, "a set's HW partial head sums live in its EW gate-f staging columns");
@@ -181,13 +182,13 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_cell_fwd_kernel(const __grid
           } else {
             ld_state<FM, W>(src, (size_t)ag.nbr[s], b, hb * 32 + c0, B, t);
           }
-          // NeurComm with feature-major state: m~ is a plain copy of the neighbours' h_seq[t]; the weight-gradient
-          // kernel reads it from there (tc_wgrad.cu), so it is not saved a second time
-          if (SAVE && !(FM && VAR == NMARL_NC)) st_fm<W>(xin_fm, xm0 + s * NH + hb * 32 + c0, B, b, t);
+          // NeurComm: m~ is a plain copy of the neighbours' h_seq[t]; the weight-gradient kernel reads it from there
+          // (tc_wgrad.cu), so it is not saved a second time
+          if (SAVE && VAR != NMARL_NC) st_fm<W>(xin_fm, xm0 + s * NH + hb * 32 + c0, B, b, t);
           produce_in(c, t);
         }
       }
-      if (SAVE && !(FM && VAR == NMARL_NC)) {
+      if (SAVE && VAR != NMARL_NC) {
         float z[W];
 #pragma unroll
         for (int j = 0; j < W; ++j) z[j] = 0.f;
@@ -247,7 +248,8 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_cell_fwd_kernel(const __grid
     }
 #pragma unroll
     for (int hb = 0; hb < 2; ++hb) {
-      if (SAVE && !FM) st_fm<W>(sh_fm, SD + hb * 32 + c0, B, b, hv[hb]);   // FM: h^ = (1 - done) * h_seq[t], re-derived by tc_wgrad
+      // outside DIAL h^ = (1 - done) * h_seq[t] is re-derived by tc_wgrad from the feature-major state sequence
+      if (SAVE && VAR == NMARL_DIAL) st_fm<W>(sh_fm, SD + hb * 32 + c0, B, b, hv[hb]);
       produce_in(c, hv[hb]);
     }
     STAMP();
@@ -430,9 +432,9 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_cell_fwd_kernel(const __grid
 
 NMARL_PARAMS_FIT(nmarl_model, FwdK);                                             // tc_cell_fwd_kernel
 
-template <int VAR, int MODE, bool FM, int HW>
-int launch_tc_fm(const nmarl_model* m, const FwdK& k, cudaStream_t st) {
-  auto kern = tc_cell_fwd_kernel<VAR, MODE, FM, HW>;
+template <int VAR, int MODE, int HW>
+int launch_tc_hw(const nmarl_model* m, const FwdK& k, cudaStream_t st) {
+  auto kern = tc_cell_fwd_kernel<VAR, MODE, HW>;
   static bool configured = false;
   if (!configured) {
     NMARL_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TC_SMEM));
@@ -444,11 +446,6 @@ int launch_tc_fm(const nmarl_model* m, const FwdK& k, cudaStream_t st) {
   NMARL_CUDA(nmarl_launch(kern, grid, dim3(TC_THREADS), TC_SMEM, st, true, *m, k2));
   NMARL_LAUNCH_CHECK();
   return 0;
-}
-
-template <int VAR, int MODE, int HW>
-int launch_tc_hw(const nmarl_model* m, const FwdK& k, cudaStream_t st) {
-  return k.a.state_fm ? launch_tc_fm<VAR, MODE, true, HW>(m, k, st) : launch_tc_fm<VAR, MODE, false, HW>(m, k, st);
 }
 
 template <int VAR, int MODE>

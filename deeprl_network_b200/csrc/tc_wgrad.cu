@@ -5,9 +5,10 @@
 //   A operand: the saved activations are feature-major ([t][agent][feature][env]); operand row = feature ka, so
 //              a thread reads the 32 consecutive envs of one k-block (one 128-byte line), splits hi/lo and stores
 //              them into the swizzled shared-memory ring.
-//   B operand: D^T, K-major over rows, was written by the backward cell kernel as ready-made [hi | lo]
-//              128B-swizzled tiles (dz: 256 rows, encoder pre-activation grads: 192/128/64 rows); one thread
-//              bulk-copies the needed row range of the tile per 32 env rows.
+//   B operand: D^T, K-major over rows, was written by the backward cell kernel as raw fp32 128B-swizzled tiles
+//              (dz: 256 rows, encoder pre-activation grads: 192/128/64 rows; nmarl_tc_tile_offset); one thread
+//              bulk-copies the needed row range of the tile per 32 env rows and the A producers split it into
+//              [hi | lo] in shared memory.
 //   Biases:    the obs-encoder job carries an extra all-ones lane and spans every column of the dpre tile, which
 //              yields all encoder bias gradients for free; the gate bias is a coalesced column sum of dz.
 #include "bwd_common.cuh"
@@ -55,7 +56,7 @@ struct RingPos {
 struct TcWgK {
   int B, T, splits, ndp;
   const float* sv_sh; const float* sv_xin; const float* dzT; const float* dpT;
-  const float* h_seq; const float* done_pre;   // feature-major state path: h^ / m~ operand rows come from the state sequence
+  const float* h_seq; const float* done_pre;   // all but DIAL (feature-major state): h^ / m~ operand rows come from h_seq
   float* ws;
   long long ws_off[J_COUNT];     // float offset of each job's partial block [splits][N_agents][128][N_job]
   int jobs[J_COUNT]; int n_jobs; // job kinds present
@@ -91,19 +92,18 @@ __device__ __forceinline__ JobDesc job_desc(const nmarl_model& m, const TcWgK& k
   return d;
 }
 
-// RAW: the D^T tiles hold raw fp32 once.  One tile per k-block is copied into the hi half of the stage; the A-producer
-// threads split it in place into the same rounded [hi | lo] pair the packed tiles carry (tc::split_tf32) and signal
-// b_split, so the split overlaps the previous k-block's MMAs instead of preceding the k-block's own.
+// The D^T tiles hold raw fp32.  One tile per k-block is copied into the hi half of the stage; the A-producer threads
+// split it in place into its rounded [hi | lo] pair (tc::split_tf32) and signal b_split, so the split overlaps the
+// previous k-block's MMAs instead of preceding the k-block's own.
 //
 // Hand-offs per k-block q (B stage st = q mod S, A slot = q mod A; every wait is on an mbarrier):
 //   thread 0 of MMA warpgroup 0 bulk-copies tile q into st once b_empty[st] reports that every active warpgroup has
-//   retired k-block q - S;  the producers fill the A slot once a_empty reports the same for q - A, then (RAW) split
-//   stage st once b_full[st] has landed;  each active MMA warpgroup waits for b_split / b_full and a_full, issues its
+//   retired k-block q - S;  the producers fill the A slot once a_empty reports the same for q - A, then split
+//   stage st once b_full[st] has landed;  each active MMA warpgroup waits for b_split and a_full, issues its
 //   12 wgmma against its own 64 A rows and the shared B stage, retires them and arrives on a_empty and b_empty (one
 //   arrival per warp, so both count 4 x the active warpgroups).
 // A warpgroup whose 64 lanes all lie beyond the job's real lanes (ka_cnt + ones lane + fingerprints) issues nothing:
 // the reduce never reads those lanes.
-template <bool RAW>
 __global__ void __launch_bounds__(WG_THREADS, 1) tc_wgrad_kernel(const __grid_constant__ nmarl_model m,
                                                                  const __grid_constant__ TcWgK k) {
   extern __shared__ uint8_t smem_raw[];
@@ -149,8 +149,8 @@ __global__ void __launch_bounds__(WG_THREADS, 1) tc_wgrad_kernel(const __grid_co
     const bool is_p = ka > d.ka_cnt && ka <= d.ka_cnt + d.p_cnt;
     const bool real = on && (ka < d.ka_cnt || is_p);
     const int feat = is_p ? d.p_feat0 + (ka - d.ka_cnt - 1) : d.a_feat0 + ka;
-    // Feature-major state path: the forward kernel does not save h^ (= (1 - done) * own h_seq[t]) and, for NeurComm,
-    // m~ (= the neighbours' h_seq[t]) a second time; those operand rows are read from the state sequence itself.
+    // Feature-major state (all but DIAL): the forward kernel does not save h^ (= (1 - done) * own h_seq[t]) and, for
+    // NeurComm, m~ (= the neighbours' h_seq[t]) a second time; those operand rows are read from the state sequence.
     int hs_agent = -1, hs_unit = 0;
     bool hs_mask = false;
     if (k.h_seq != nullptr && real && !is_p) {
@@ -209,24 +209,22 @@ __global__ void __launch_bounds__(WG_THREADS, 1) tc_wgrad_kernel(const __grid_co
       tc::mbar_arrive(&a_full[as.idx]);
       as.next(AS);
       if (q + 2 < nkb) load_x(q + 2, x);        // refill this buffer; it is consumed two k-blocks from now
-      if constexpr (RAW) {
-        // split the raw D^T tile of this k-block into its [hi | lo] pair once it has landed.  In order: the stage is
-        // refilled with k-block q + S only after the MMAs of q, which wait for this split, have retired.
-        tc::mbar_wait(&b_full[bs.idx], bs.ph, k.err, 31);
-        float4* bhi = reinterpret_cast<float4*>(bst + (size_t)bs.idx * 2 * tile_bytes);
-        float4* blo = reinterpret_cast<float4*>(bst + (size_t)bs.idx * 2 * tile_bytes + tile_bytes);
-        for (uint32_t e = (uint32_t)tid; e < tile_bytes / 16; e += WG_A_THREADS) {
-          const float4 v = bhi[e];
-          float4 h, lo4;
-          tc::split_tf32(v.x, h.x, lo4.x); tc::split_tf32(v.y, h.y, lo4.y);
-          tc::split_tf32(v.z, h.z, lo4.z); tc::split_tf32(v.w, h.w, lo4.w);
-          bhi[e] = h;
-          blo[e] = lo4;
-        }
-        tc::fence_proxy_async();
-        tc::mbar_arrive(&b_split[bs.idx]);
-        bs.next(S);
+      // split the raw D^T tile of this k-block into its [hi | lo] pair once it has landed.  In order: the stage is
+      // refilled with k-block q + S only after the MMAs of q, which wait for this split, have retired.
+      tc::mbar_wait(&b_full[bs.idx], bs.ph, k.err, 31);
+      float4* bhi = reinterpret_cast<float4*>(bst + (size_t)bs.idx * 2 * tile_bytes);
+      float4* blo = reinterpret_cast<float4*>(bst + (size_t)bs.idx * 2 * tile_bytes + tile_bytes);
+      for (uint32_t e = (uint32_t)tid; e < tile_bytes / 16; e += WG_A_THREADS) {
+        const float4 v = bhi[e];
+        float4 h, lo4;
+        tc::split_tf32(v.x, h.x, lo4.x); tc::split_tf32(v.y, h.y, lo4.y);
+        tc::split_tf32(v.z, h.z, lo4.z); tc::split_tf32(v.w, h.w, lo4.w);
+        bhi[e] = h;
+        blo[e] = lo4;
       }
+      tc::fence_proxy_async();
+      tc::mbar_arrive(&b_split[bs.idx]);
+      bs.next(S);
     };
     if (nkb > 0) load_x(0, xa);
     if (nkb > 1) load_x(1, xb);
@@ -251,16 +249,10 @@ __global__ void __launch_bounds__(WG_THREADS, 1) tc_wgrad_kernel(const __grid_co
     auto fetch = [&](int q, int st) {
       const int kb = kb0 + q;
       const int tt = kb / bpt, rb = kb - tt * bpt;
-      // byte offset of the D^T tile of (t, 32-env block rb): [hi | lo] pairs, or single raw tiles packed inside each
-      // time step's (unchanged) [hi | lo]-sized slab
-      const size_t pair = (size_t)(2 * d.tile_rows * 128);
-      const size_t off = RAW ? (size_t)tt * N_agents * bpt * pair + ((size_t)i * bpt + rb) * (pair / 2)
-                             : (((size_t)tt * N_agents + i) * bpt + rb) * pair;
-      const uint8_t* tile = reinterpret_cast<const uint8_t*>(d.BT) + off;
-      uint8_t* dst = bst + (size_t)st * 2 * tile_bytes;
-      tc::mbar_arrive_expect_tx(&b_full[st], RAW ? tile_bytes : 2 * tile_bytes);
+      const uint8_t* tile = reinterpret_cast<const uint8_t*>(d.BT + nmarl_tc_tile_offset(d.tile_rows, tt, N_agents, bpt, i, rb));
+      uint8_t* dst = bst + (size_t)st * 2 * tile_bytes;         // the raw tile lands in the hi half of the stage
+      tc::mbar_arrive_expect_tx(&b_full[st], tile_bytes);
       tc::bulk_g2s(dst, tile + (size_t)d.n_row0 * 128, tile_bytes, &b_full[st]);
-      if (!RAW) tc::bulk_g2s(dst + tile_bytes, tile + (size_t)(d.tile_rows + d.n_row0) * 128, tile_bytes, &b_full[st]);
     };
     if (issuer)
       for (int q = 0; q < S && q < nkb; ++q) fetch(q, q);
@@ -284,8 +276,7 @@ __global__ void __launch_bounds__(WG_THREADS, 1) tc_wgrad_kernel(const __grid_co
     for (int q = 0; q < nkb; ++q) {
       const bool seg_first = (q % SEG_KB) == 0;
       uint8_t* b = bst + (size_t)bs.idx * 2 * tile_bytes;
-      if constexpr (RAW) tc::mbar_wait(&b_split[bs.idx], bs.ph, k.err, 33);   // landed and split (A producers)
-      else tc::mbar_wait(&b_full[bs.idx], bs.ph, k.err, 31);
+      tc::mbar_wait(&b_split[bs.idx], bs.ph, k.err, 33);      // landed and split (A producers)
       if (prof && q < 300) prof[4 + 3 * q] = clock64();
       tc::mbar_wait(&a_full[as.idx], as.ph, k.err, 32);
       if (prof && q < 300) prof[5 + 3 * q] = clock64();
@@ -396,7 +387,7 @@ int64_t nmarl_tc_wgrad_ws_floats(const nmarl_model* m) {
 
 int nmarl_tc_launch_wgrads(const nmarl_model* m, int B, int T, const float* sv_sh, const float* sv_xin, const float* dzT,
                            const float* dpT, const float* sv_dz, float* ws, float* grads, int* err, cudaStream_t st,
-                           cudaStream_t st_bias, bool raw_tiles, void** ev_wgrad, const float* h_seq, const float* done_pre) {
+                           cudaStream_t st_bias, void** ev_wgrad, const float* h_seq, const float* done_pre) {
   TcWgK k{};
   k.B = B; k.T = T; k.splits = nmarl_tc_wgrad_splits(m->n_agent); k.ndp = nmarl_tc_ndp(m);
   k.sv_sh = sv_sh; k.sv_xin = sv_xin; k.dzT = dzT; k.dpT = dpT; k.ws = ws; k.err = err;
@@ -406,8 +397,7 @@ int nmarl_tc_launch_wgrads(const nmarl_model* m, int B, int T, const float* sv_s
   for (int j = 0; j < k.n_jobs; ++j) { k.ws_off[j] = off; off += (long long)k.splits * m->n_agent * 128 * job_N(m, k.jobs[j]); }
   static bool configured = false;
   if (!configured) {
-    NMARL_CUDA(cudaFuncSetAttribute(tc_wgrad_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)WG_SMEM));
-    NMARL_CUDA(cudaFuncSetAttribute(tc_wgrad_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)WG_SMEM));
+    NMARL_CUDA(cudaFuncSetAttribute(tc_wgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)WG_SMEM));
     configured = true;
   }
   // independent of the GEMM jobs; the backward cell kernel leaves one partial per 32 env rows
@@ -415,8 +405,7 @@ int nmarl_tc_launch_wgrads(const nmarl_model* m, int B, int T, const float* sv_s
   NMARL_LAUNCH_CHECK();
   if (ev_wgrad) NMARL_CUDA(cudaEventRecord((cudaEvent_t)ev_wgrad[0], st));
   const dim3 grid(k.splits, k.n_jobs, m->n_agent);                   // one CTA per (row split, 128-lane job tile, agent)
-  if (raw_tiles) tc_wgrad_kernel<true><<<grid, WG_THREADS, WG_SMEM, st>>>(*m, k);
-  else tc_wgrad_kernel<false><<<grid, WG_THREADS, WG_SMEM, st>>>(*m, k);
+  tc_wgrad_kernel<<<grid, WG_THREADS, WG_SMEM, st>>>(*m, k);
   NMARL_LAUNCH_CHECK();
   if (ev_wgrad) NMARL_CUDA(cudaEventRecord((cudaEvent_t)ev_wgrad[1], st));
   NMARL_DBG_SYNC(st, "tc_wgrad_kernel");

@@ -956,6 +956,11 @@ int run_wgrad(const nmarl_model* m, const nmarl_bwd_args* a, int nd, const float
   return 0;
 }
 
+// tensor cores: whole 128-env tiles, narrow encoders and the width the wgmma kernels are built for (NMARL_NH)
+bool bptt_tc_path(const nmarl_model* m, const nmarl_bwd_args* a) {
+  return a->wpack != nullptr && a->B % 128 == 0 && m->kx_pad <= 32 && m->kp_pad <= 32 && nmarl_n_h(*m) == NMARL_NH;
+}
+
 int check_bwd_args(const nmarl_model* m, const nmarl_bwd_args* a) {
   if (nmarl_check_model(m)) return 1;
   NMARL_CHECK(a && a->B > 0 && a->T > 0 && a->B_total >= a->B, "a2c_backward: bad sizes");
@@ -967,8 +972,7 @@ int check_bwd_args(const nmarl_model* m, const nmarl_bwd_args* a) {
   NMARL_CHECK(m->variant == NMARL_IA2C || a->dmsg, "a2c_backward: dmsg buffer required");
   NMARL_CHECK((m->variant != NMARL_IC3 && m->variant != NMARL_DIAL) || a->sv_enc, "a2c_backward: sv_enc required");
   NMARL_CHECK(m->variant != NMARL_DIAL || (a->msg_seq && a->sv_dmp), "a2c_backward: DIAL buffers required");
-  NMARL_CHECK(!a->state_fm || (m->variant != NMARL_DIAL && a->wpack != nullptr && a->B % 128 == 0 && nmarl_n_h(*m) == NMARL_NH),
-              "a2c_backward: feature-major state needs the tensor-core path (and is not implemented for DIAL)");
+  NMARL_CHECK(a->state_fm == nmarl_state_fm(m, bptt_tc_path(m, a)), "a2c_backward: " NMARL_STATE_FM_RULE, a->state_fm);
   NMARL_CHECK((m->variant != NMARL_NC && m->variant != NMARL_DIAL) || a->fp, "a2c_backward: fp required");
   return 0;
 }
@@ -1079,8 +1083,7 @@ extern "C" int nmarl_a2c_bptt(const nmarl_model* m, const nmarl_bwd_args* a, voi
   // 1. transposed weights for the FFMA backward kernels and DIAL's message-gradient kernel (the tensor-core cell
   //    kernels read their own packed transposed operands, refreshed by nmarl_pack_weights)
   //    One launch covers every agent.
-  // tensor cores: whole 128-env tiles, narrow encoders and the width the wgmma kernels are built for (NMARL_NH)
-  const bool tc_path = (a->wpack != nullptr && B % 128 == 0 && m->kx_pad <= 32 && m->kp_pad <= 32 && H == NMARL_NH);
+  const bool tc_path = bptt_tc_path(m, a);
   if (!tc_path || m->variant == NMARL_DIAL) {
     const int jobs = NMARL_TJ_WXH | (m->variant != NMARL_IA2C ? NMARL_TJ_MSG : 0) | (m->variant == NMARL_DIAL ? NMARL_TJ_MFC : 0);
     if (nmarl_launch_transposes(m, jobs, a->params, a->wt, st)) return 1;
@@ -1112,7 +1115,6 @@ extern "C" int nmarl_a2c_bptt(const nmarl_model* m, const nmarl_bwd_args* a, voi
   }
   NMARL_CUDA(cudaEventRecord(ev_join, side));
   // 2. reverse time
-  const int raw_tiles = a->raw_tiles ? 1 : 0;      // single-copy operand tiles (DESIGN.md)
   for (int t = T - 1; t >= 0; --t) {
     BwdK k{};
     k.B = B; k.t = t; k.has_next = (t < T - 1);
@@ -1133,13 +1135,12 @@ extern "C" int nmarl_a2c_bptt(const nmarl_model* m, const nmarl_bwd_args* a, voi
     }
     k.sv_dpre = a->sv_dpre + (size_t)t * nb * (3 * H);
     k.wpack = a->wpack; k.tc_err = a->tc_err; k.state_fm = a->state_fm;
-    k.raw_tiles = raw_tiles;
     const bool use_tc = tc_path;
     // tensor-core path: sv_dz holds the gate-bias partial sums of every 32 env rows [T][N][B/32][256]; FFMA path: dz [T][N][B][256]
     k.sv_dz = use_tc ? a->sv_dz + (size_t)t * N * (B / 32) * (4 * H) : a->sv_dz + (size_t)t * nb * (4 * H);
-    k.dzT = (use_tc && a->sv_dzT) ? a->sv_dzT + (size_t)t * N * (B / 32) * (2 * 256 * 32) : nullptr;
+    k.dzT = (use_tc && a->sv_dzT) ? a->sv_dzT + nmarl_tc_tile_offset(NG, t, N, B / 32, 0, 0) : nullptr;
     k.ndp = nmarl_tc_ndp(m);
-    k.dpT = (use_tc && a->sv_dpT) ? a->sv_dpT + (size_t)t * N * (B / 32) * (2 * k.ndp * 32) : nullptr;
+    k.dpT = (use_tc && a->sv_dpT) ? a->sv_dpT + nmarl_tc_tile_offset(k.ndp, t, N, B / 32, 0, 0) : nullptr;
     int rc = 0;
     if (t == T - 1 - lead) NMARL_CUDA(cudaStreamWaitEvent(st, a->ctx->heads, 0));   // dlv of steps < T - lead
     if (a->ev_step) NMARL_CUDA(cudaEventRecord((cudaEvent_t)a->ev_step[2 * t], st));
@@ -1170,7 +1171,7 @@ extern "C" int nmarl_a2c_bptt(const nmarl_model* m, const nmarl_bwd_args* a, voi
     // the gate-bias column sums only read sv_dz: second fork, beside the GEMM jobs
     NMARL_CUDA(cudaEventRecord(ev_fork, st));
     NMARL_CUDA(cudaStreamWaitEvent(side, ev_fork, 0));
-    if (nmarl_tc_launch_wgrads(m, B, T, a->sv_sh, a->sv_xin, a->sv_dzT, a->sv_dpT, a->sv_dz, a->ws, a->grads, a->tc_err, st, side, raw_tiles != 0, a->ev_wgrad,
+    if (nmarl_tc_launch_wgrads(m, B, T, a->sv_sh, a->sv_xin, a->sv_dzT, a->sv_dpT, a->sv_dz, a->ws, a->grads, a->tc_err, st, side, a->ev_wgrad,
                                a->state_fm ? a->h_seq : nullptr, a->done_pre)) return 1;
     NMARL_CUDA(cudaEventRecord(ev_join, side));
     NMARL_CUDA(cudaStreamWaitEvent(st, ev_join, 0));

@@ -172,7 +172,8 @@ typedef struct {
   /* optional (p-call, tensor-core path only): save the activations BPTT needs while rolling out, so the
    * update can skip the separate training forward (same inputs, same weights => same numbers):         */
   float* sv_xin; float* sv_sh; float* sv_gates; float* sv_enc;   /* step-t slices, see nmarl_bwd_args      */
-  int32_t state_fm;        /* tensor-core path only: c/h/msg tensors are feature-major [N][64][B]   */
+  int32_t state_fm;        /* layout of c/h: 1 = feature-major [N][64][B], required on the tensor-  */
+                           /* core path except for DIAL; 0 = env-major, required everywhere else */
 } nmarl_fwd_args;
 
 int nmarl_policy_step_p(const nmarl_model* m, const nmarl_fwd_args* a, void* stream);
@@ -237,19 +238,17 @@ typedef struct {
   float* grads;
   const float* wpack;        /* packed tensor-core operands or NULL (see nmarl_fwd_args)            */
   int32_t* tc_err;
-  float* sv_dzT;             /* tensor-core path: dz^T as [T][N][B/32][hi|lo][256][32] swizzled tiles  */
-  float* sv_dpT;             /* tensor-core path: encoder pre-activation grads^T, [T][N][B/32][hi|lo][ndp][32],
-                                ndp = 192 (NC) / 128 (IC3, DIAL) / 64 (IA2C).  On the tensor-core path (wpack set,
-                                B % 128 == 0) sv_xin / sv_sh / sv_gates / sv_enc are FEATURE-MAJOR
+  float* sv_dzT;             /* tensor-core path: dz^T as [T][N][B/32][256][32], one raw fp32 128B-swizzled tile per
+                                32 env rows (the weight-gradient kernel splits it into 3xTF32 hi / lo itself)        */
+  float* sv_dpT;             /* tensor-core path: encoder pre-activation grads^T, [T][N][B/32][ndp][32] raw tiles
+                                like sv_dzT, ndp = 192 (NC) / 128 (IC3, DIAL) / 64 (IA2C).  On the tensor-core path
+                                (wpack set, B % 128 == 0) sv_xin / sv_sh / sv_gates / sv_enc are FEATURE-MAJOR
                                 [T][N][feature][B] and sv_dpre is unused.  With state_fm the done-masked own state
                                 (rows s_dim.. of sv_sh) and, for NeurComm, the neighbour messages (the m~ block of
                                 sv_xin) are NOT stored a second time: the weight-gradient kernel reads h_seq.        */
-  int32_t state_fm;          /* tensor-core path only: h_seq / c_seq / msg_seq / dh_rec / dc_rec / dmsg are
-                                feature-major ([..][64][B] instead of [..][B][64])                                  */
+  int32_t state_fm;          /* h_seq / c_seq / msg_seq / dh_rec / dc_rec / dmsg are feature-major ([..][64][B]
+                                instead of [..][B][64]): 1 on the tensor-core path except for DIAL, else 0           */
   nmarl_ctx* ctx;            /* required by nmarl_a2c_bptt / nmarl_a2c_backward (forked side work)                  */
-  int32_t raw_tiles;         /* tensor-core path: sv_dzT / sv_dpT hold ONE raw fp32 tile per 32 rows (the weight-
-                                gradient kernel derives the 3xTF32 `lo` part in shared memory) instead of a
-                                [hi | lo] pair: half the operand-tile traffic                                       */
   void** ev_step;            /* optional timing hooks (bench.py): 2*T cudaEvent_t, recorded on `stream` before /
                                 after the cell kernel of reverse step t at [2t], [2t+1]; NULL = none               */
   void** ev_wgrad;           /* optional: 2 cudaEvent_t around the weight-gradient GEMM kernel; NULL = none         */
@@ -257,6 +256,8 @@ typedef struct {
 
 int nmarl_loss_tiles(const nmarl_model* m, int B);       /* tiles per agent in loss_part      */
 int64_t nmarl_ws_floats(const nmarl_model* m, int B, int T);   /* required workspace          */
+/* float offset in sv_dzT (rows = 256) or sv_dpT (rows = ndp) of the tile of time step t, agent, 32-env block */
+int64_t nmarl_operand_tile_offset(int rows, int t, int n_agent, int B, int agent, int block);
 int nmarl_a2c_backward(const nmarl_model* m, const nmarl_bwd_args* a, void* stream);
 /* the two halves: the training forward re-runs the T cell steps from states_bw and saves the activations
  * (sv_xin, sv_sh, sv_gates, sv_enc) and h_seq / c_seq / msg_seq.  nmarl_a2c_bptt computes the heads, the loss

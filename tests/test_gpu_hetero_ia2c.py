@@ -6,8 +6,8 @@
     neighbours' policies appended to every observation), from the same NumPy-stream initial weights (exact): every
     pi / v / R within 1e-5, the sampled trained weights within 2e-5, and after the three updates every padding float of
     the embedding is still exactly 0 (the padded actions' -1e30 biases unchanged).
-(2) Batched kernels against the float64 oracle (tests/hetero_ia2c_oracle.py): B = 7 (FP32-FFMA) and B = 128 (tensor
-    cores, every state layout and operand-tile setting, tc_err == 0).  States, loss terms and every gradient entry are
+(2) Batched kernels against the float64 oracle (tests/hetero_ia2c_oracle.py): B = 7 (FP32-FFMA), B = 128 and
+    B = 256 (tensor cores: one and two 128-env tiles per agent, feature-major state, tc_err == 0).  States, loss terms and every gradient entry are
     judged with the round-off scale of tests/test_gpu_tc_paths.py, the padding gets exactly zero gradient; then two
     optimizer steps: per-group norm_out, the weights and the untouched padding.
 (3) IA2C_CU: nmarl_consensus_update alone (zero gradients) gives the oracle's consensus_update of the LSTM blocks and
@@ -114,29 +114,26 @@ def _oracle(agent, params, c, x, n_s, n_a, mask):
 
 
 @pytest.mark.parametrize('name', GOLDEN)
-@pytest.mark.parametrize('B', [7, 128])                     # 128: tensor-core path
-def test_hetero_ia2c_kernels_match_oracle(name, B, monkeypatch):
+@pytest.mark.parametrize('B', [7, 128, 256])                # 128, 256: tensor-core path
+def test_hetero_ia2c_kernels_match_oracle(name, B):
     agent, lay, params, c, n_s, n_a = _setup(name, B)
     x = _inputs(c, n_s, n_a, seed=1)
     W, used, pad = max(n_s), _used(lay), _padding(lay)
     tc = B % 128 == 0
-    configs = [(fm, raw) for fm in (True, False) for raw in (True, False)] if tc else [(False, False)]
-    for fm, raw in configs:
-        tag = 'B=%d state_fm=%d raw_tiles=%d' % (B, fm, raw)
-        e = _engine(lay, params, c, monkeypatch, tc=tc, fm=fm, raw=raw)
-        r = _run(e, agent, lay, x, W)                        # _result: synchronize + check_tc (tc_err == 0)
-        orc, ref = _oracle(agent, params, c, x, n_s, n_a, lay.mask)
-        ratios = _check(tag, r, ref, used)
-        if tc:                                               # per-entry error within 4x the FFMA kernels' + FLOOR
-            e0 = _engine(lay, params, c, monkeypatch, tc=False)
-            r0 = _check(tag + ' ffma', _run(e0, agent, lay, x, W), ref, used)
-            del e0
-            bad = {n: (ratios[n], r0[n]) for n in ratios if ratios[n] > 4 * r0[n] + FLOOR}
-            assert not bad, (tag, sorted(bad.items(), key=lambda t: -t[1][0])[:6])
-        assert e.norm_out.numel() == (len(n_s) if agent != 'ma2c_cu' else 1)
-        check_apply_twice(e, orc, lay, pad)
-        e.check_tc()
-        del e
+    tag = 'B=%d' % B
+    e = _engine(lay, params, c, tc=tc)
+    r = _run(e, agent, lay, x, W)                            # _result: synchronize + check_tc (tc_err == 0)
+    orc, ref = _oracle(agent, params, c, x, n_s, n_a, lay.mask)
+    ratios = _check(tag, r, ref, used)
+    if tc:                                                   # per-entry error within 4x the FFMA kernels' + FLOOR
+        e0 = _engine(lay, params, c, tc=False)
+        r0 = _check(tag + ' ffma', _run(e0, agent, lay, x, W), ref, used)
+        del e0
+        bad = {n: (ratios[n], r0[n]) for n in ratios if ratios[n] > 4 * r0[n] + FLOOR}
+        assert not bad, (tag, sorted(bad.items(), key=lambda t: -t[1][0])[:6])
+    assert e.norm_out.numel() == (len(n_s) if agent != 'ma2c_cu' else 1)
+    check_apply_twice(e, orc, lay, pad)
+    e.check_tc()
 
 
 @pytest.mark.parametrize('name', [p for p in GOLDEN if p.values[0].endswith('ma2c_cu')])

@@ -106,11 +106,10 @@ def _mask(shape):
     return grid_masks(8)[0] if shape == 'grid8x8' else chain_masks(128)[0]
 
 
-def _engine(lay, params, B, T, monkeypatch, fm=True, raw=True):
+def _engine(lay, params, B, T):
     from deeprl_network_b200.agents.engine import PolicyEngine
-    monkeypatch.setenv('NMARL_NO_STATE_FM', '0' if fm else '1')
     eng = PolicyEngine(lay, B, T, dict(HP), flat_params=lay.pack(params))
-    eng.raw_tiles = eng.use_tc and raw
+    assert eng.state_fm == (eng.use_tc and eng.variant != 'ma2c_dial'), 'feature-major state on tensor cores, but DIAL'
     return eng
 
 
@@ -130,7 +129,7 @@ def _check_grad(tag, n, g, ref):
 @pytest.mark.parametrize('B', [7, 128])                                  # 7: FP32 FFMA, 128: tensor cores
 @pytest.mark.parametrize('shape', ['grid8x8', 'chain128'])
 @pytest.mark.parametrize('variant', VARIANTS)
-def test_many_agent_kernels_match_oracle(variant, shape, B, monkeypatch):
+def test_many_agent_kernels_match_oracle(variant, shape, B):
     from deeprl_network_b200.layout import ModelLayout
     T = 3
     mask = _mask(shape)
@@ -157,42 +156,38 @@ def test_many_agent_kernels_match_oracle(variant, shape, B, monkeypatch):
     orc.states_bw, orc.states_fw = st.clone(), st.clone()
     orc.backward(obs_o, fp.astype(np.float64), acts, dones, Rs, Advs, 5e-4, v_coef=HP['v_coef'], e_coef=HP['e_coef'],
                  apply=False)
-    configs = [(True, True), (True, False), (False, True), (False, False)] if B == 128 else [(True, True)]
-    if variant == 'ma2c_dial' and B == 128:          # DIAL keeps env-major state
-        configs = [(True, True), (True, False)]
     pad = np.ones(lay.n_param, bool)
     for _, o, s in lay.entries:
         pad[o:o + int(np.prod(s))] = False
-    for fm, raw in configs:
-        tag = '%s %s B=%d state_fm=%d raw_tiles=%d' % (variant, shape, B, fm, raw)
-        eng = _engine(lay, params, B, T, monkeypatch, fm, raw)
-        assert eng.use_tc == (B == 128), tag
-        # ---- forward p / v ----
-        eng.set_states(nb(c0), nb(h0))
-        obs_d = torch.zeros(N, B, lay.obs_stride, device='cuda'); obs_d[:, :, :5] = nb(base[0])
-        pi_d = torch.zeros(N, B, N_A, device='cuda'); v_d = torch.zeros(N, B, device='cuda')
-        eng.step_p(obs_d, nb(fp[0]), to_dev(dones[0]), pi_d)
-        np.testing.assert_allclose(bn(pi_d), pi_o, rtol=0, atol=1e-5, err_msg=tag)
-        np.testing.assert_allclose(bn(eng.get_states_fw()), st_o, rtol=0, atol=1e-5, err_msg=tag)
-        eng.step_v(obs_d, nb(fp[0]), to_dev(dones[0]), nb(acts[0]).int(), v_d)
-        np.testing.assert_allclose(bn(v_d), v_o, rtol=0, atol=1e-5, err_msg=tag)
-        # ---- backward ----
-        eng.T_cur = T
-        eng.obs_buf[:T].zero_(); eng.obs_buf[:T, :, :, :5].copy_(to_dev(np.transpose(base, (0, 2, 1, 3))))
-        eng.fp_buf[:T].copy_(to_dev(np.transpose(fp, (0, 2, 1, 3))))
-        eng.act_buf[:T].copy_(to_dev(np.transpose(acts, (0, 2, 1)), torch.int32))
-        eng.done_buf[:T].copy_(to_dev(dones))
-        eng.Rs[:T].copy_(to_dev(np.transpose(Rs, (0, 2, 1)))); eng.Advs[:T].copy_(to_dev(np.transpose(Advs, (0, 2, 1))))
-        eng.set_states(nb(c0), nb(h0))
-        eng.backward()
-        torch.cuda.synchronize()
-        eng.check_tc()
-        flat = eng.grads.cpu().numpy()
-        gk = lay.unpack(flat)
-        for n in orc.names:
-            _check_grad(tag, n, gk[n], orc.grads[n].numpy())
-        assert np.all(flat[pad] == 0), tag                    # the layout padding gets exactly zero gradient
-    # ---- two optimizer steps (last configuration); IA2C / IA2C_FP: one norm per agent ----
+    tag = '%s %s B=%d' % (variant, shape, B)
+    eng = _engine(lay, params, B, T)
+    assert eng.use_tc == (B == 128), tag
+    # ---- forward p / v ----
+    eng.set_states(nb(c0), nb(h0))
+    obs_d = torch.zeros(N, B, lay.obs_stride, device='cuda'); obs_d[:, :, :5] = nb(base[0])
+    pi_d = torch.zeros(N, B, N_A, device='cuda'); v_d = torch.zeros(N, B, device='cuda')
+    eng.step_p(obs_d, nb(fp[0]), to_dev(dones[0]), pi_d)
+    np.testing.assert_allclose(bn(pi_d), pi_o, rtol=0, atol=1e-5, err_msg=tag)
+    np.testing.assert_allclose(bn(eng.get_states_fw()), st_o, rtol=0, atol=1e-5, err_msg=tag)
+    eng.step_v(obs_d, nb(fp[0]), to_dev(dones[0]), nb(acts[0]).int(), v_d)
+    np.testing.assert_allclose(bn(v_d), v_o, rtol=0, atol=1e-5, err_msg=tag)
+    # ---- backward ----
+    eng.T_cur = T
+    eng.obs_buf[:T].zero_(); eng.obs_buf[:T, :, :, :5].copy_(to_dev(np.transpose(base, (0, 2, 1, 3))))
+    eng.fp_buf[:T].copy_(to_dev(np.transpose(fp, (0, 2, 1, 3))))
+    eng.act_buf[:T].copy_(to_dev(np.transpose(acts, (0, 2, 1)), torch.int32))
+    eng.done_buf[:T].copy_(to_dev(dones))
+    eng.Rs[:T].copy_(to_dev(np.transpose(Rs, (0, 2, 1)))); eng.Advs[:T].copy_(to_dev(np.transpose(Advs, (0, 2, 1))))
+    eng.set_states(nb(c0), nb(h0))
+    eng.backward()
+    torch.cuda.synchronize()
+    eng.check_tc()
+    flat = eng.grads.cpu().numpy()
+    gk = lay.unpack(flat)
+    for n in orc.names:
+        _check_grad(tag, n, gk[n], orc.grads[n].numpy())
+    assert np.all(flat[pad] == 0), tag                        # the layout padding gets exactly zero gradient
+    # ---- two optimizer steps; IA2C / IA2C_FP: one norm per agent ----
     assert eng.norm_out.numel() == (N if variant in ('ia2c', 'ia2c_fp') else 1)
     check_apply_twice(eng, orc, lay, pad)
     assert int(eng.tc_err.item()) == 0

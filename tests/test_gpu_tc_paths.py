@@ -1,18 +1,16 @@
-"""GPU: every instantiation of the tensor-core training step against one float64 oracle per case.
+"""GPU: both modes of the tensor-core training step against one float64 oracle per case and mode.
 
-The tensor-core kernels are templates whose instantiation is chosen at run time: the LSTM state feature-major or
-env-major (`state_fm`, NMARL_NO_STATE_FM=1), the weight-gradient operand tiles raw or as packed [hi | lo] pairs
-(`raw_tiles`), and the training forward either run by `backward()` on recorded buffers (unfused) or saved by the
-rollout p-calls and folded into the BPTT call (fused: `rollout(sample='uniform')` on a scripted env, then `backward()`).
-Per case, one set of inputs and one float64 oracle (oracle/nets.py autograd) judge every applicable configuration:
+The LSTM state layout follows from the variant (feature-major, DIAL env-major), and the training forward either runs
+in `backward()` on recorded buffers (unfused) or is saved by the rollout p-calls and folded into the BPTT call (fused:
+`rollout(sample='uniform')` on a scripted env, then `backward()`).  Each case runs in both modes, as separate
+parameter sets; one set of inputs and a float64 oracle (oracle/nets.py autograd) of the trajectory the mode ran judge
 pi / v / states, the loss terms, every gradient, and zero gradient on the layout padding.
 
 Gradients are judged per entry as well as per tensor.  A weight used as x @ W gets the round-off scale
 S_W = sum over its uses of |x|^T |delta| (delta = the gradient of the product), a bias S_b = sum |delta|; both are
 collected from the oracle's own backward.  The tensor-core error max|g - g64| / S of a tensor must stay within 4x that
 of the FP32-FFMA kernels (use_tc=False) on the same buffers plus FLOOR, so a few wrong lanes cannot hide behind the
-largest entry of their tensor.  Configurations that differ only in layout or in where the hi/lo split happens must
-agree bit for bit.
+largest entry of their tensor.
 """
 import numpy as np
 import pytest
@@ -238,13 +236,11 @@ def _inputs(c, n_s, n_a, seed=0):
     return x
 
 
-def _engine(lay, params, c, monkeypatch, tc, fm=True, raw=True):
+def _engine(lay, params, c, tc):
     from deeprl_network_b200.agents.engine import PolicyEngine
-    monkeypatch.setenv('NMARL_NO_STATE_FM', '0' if fm else '1')
     e = PolicyEngine(lay, c['B'], c['T'], dict(HP), flat_params=lay.pack(params), use_tc=tc)
     assert e.use_tc == tc, 'the shape must select the path under test'
-    assert e.state_fm == (tc and fm and e.variant != 'ma2c_dial')
-    e.raw_tiles = tc and raw
+    assert e.state_fm == (tc and e.variant != 'ma2c_dial'), 'feature-major state on the tensor-core path, but DIAL'
     return e
 
 
@@ -267,7 +263,7 @@ def _result(e, lay):
     torch.cuda.synchronize()
     e.check_tc()
     flat = e.grads.cpu().numpy()
-    return dict(flat=flat, grads=e.grads.clone(), g=lay.unpack(flat), losses=e.losses())
+    return dict(flat=flat, g=lay.unpack(flat), losses=e.losses())
 
 
 def _run_unfused(e, lay, x, fp, acts, W):
@@ -298,7 +294,7 @@ def _run_fused(e, lay, x, W):
     assert e.saved_rollout, 'the fused path (rollout p-calls save the BPTT activations) must be the one under test'
     torch.cuda.synchronize()
     rec = dict(fp=np.transpose(e.fp_buf.cpu().numpy(), (0, 2, 1, 3)), acts=np.transpose(e.act_buf.cpu().numpy(), (0, 2, 1)),
-               v=np.transpose(e.val_buf.cpu().numpy(), (0, 2, 1)), act_dev=e.act_buf.clone())
+               v=np.transpose(e.val_buf.cpu().numpy(), (0, 2, 1)))
     np.testing.assert_array_equal(e.done_buf.cpu().numpy(), x['dones'])
     c, h = _states(e, 1, T + 1)
     # the rollout's Rs / Advs come from zero rewards; the test's own values make the policy loss non-trivial
@@ -341,11 +337,6 @@ def _oracle(lay, orc_args, params, c, x, n_s, fp, acts):
                 summ=summ, pi=orc.last_pi.numpy(), v_roll=np.stack(vs), c=np.stack(cs), h=np.stack(hs))
 
 
-def _span(lay, n):
-    o, shape = lay.by_name[n]
-    return o, o + int(np.prod(shape))
-
-
 def _used(lay):
     used = np.zeros(lay.n_param, bool)
     if getattr(lay, 'hetero', False):
@@ -380,8 +371,9 @@ def _check(tag, r, ref, used):
     return ratios
 
 
+@pytest.mark.parametrize('mode', ['unfused', 'fused'])
 @pytest.mark.parametrize('c', CASES)
-def test_tc_paths_match_fp64(c, monkeypatch):
+def test_tc_paths_match_fp64(c, mode):
     lay, orc_args, n_s, n_a = _model(c)
     B, T, N = c['B'], c['T'], lay.N
     if c['kb'] is not None:            # the weight-gradient regime the case is named after
@@ -398,46 +390,19 @@ def test_tc_paths_match_fp64(c, monkeypatch):
     x = _inputs(c, n_s, n_a)
     W = max(n_s)
     used = _used(lay)
-    configs = [(fm, raw) for fm in ((True, False) if c['variant'] != 'ma2c_dial' else (False,)) for raw in (True, False)]
-    report = []
-    for mode in ('unfused', 'fused'):
-        runs = {}
-        for fm, raw in configs:
-            e = _engine(lay, params, c, monkeypatch, tc=True, fm=fm, raw=raw)
-            runs[fm, raw] = _run_unfused(e, lay, x, x['fp'], x['acts'], W) if mode == 'unfused' else _run_fused(e, lay, x, W)
-            del e
-        first = runs[configs[0]]
-        fp, acts = (x['fp'], x['acts']) if mode == 'unfused' else (first['fp'][:T], first['acts'])
-        if mode == 'fused':            # all configurations recorded the same trajectory: one oracle judges them all
-            for k in configs[1:]:
-                assert torch.equal(runs[k]['act_dev'], first['act_dev']), (mode, k, 'sampled actions differ')
-        ref = _oracle(lay, orc_args, params, c, x, n_s, fp, acts)
-        # calibration: the FP32-FFMA kernels on the same buffers against the same oracle
-        e = _engine(lay, params, c, monkeypatch, tc=False)
-        ffma = _run_unfused(e, lay, x, fp, acts, W)
-        del e
-        r_ffma = _check('%s ffma' % mode, ffma, ref, used)
-        worst_tc = 0.0
-        for k, r in runs.items():
-            tag = '%s state_fm=%d raw_tiles=%d' % (mode, k[0], k[1])
-            r_tc = _check(tag, r, ref, used)
-            bad = {n: (r_tc[n], r_ffma[n]) for n in r_tc if r_tc[n] > 4 * r_ffma[n] + FLOOR}
-            assert not bad, (tag, 'per-entry error / round-off scale', sorted(bad.items(), key=lambda t: -t[1][0])[:6])
-            worst_tc = max(worst_tc, max(r_tc.values()))
-        # raw and packed operand tiles feed the wgrad MMAs the same tc::split_tf32 pair: bit-identical gradients.
-        # The feature-major and env-major state layouts run the same cell arithmetic: bit-identical states and gradients,
-        # except pi/w and v/w -- head_wgrad_kernel (train.cu) reduces the rows of h in a layout-dependent order
-        # (32-env shuffle trees when h is feature-major, unit lanes otherwise); those are held to the oracle above.
-        heads = np.zeros(lay.n_param, bool)
-        for n in ref['g']:
-            if n.split('/')[-2].startswith(('pi', 'v')):
-                heads[lay._idx[n] if getattr(lay, 'hetero', False) else slice(*_span(lay, n))] = True
-        heads = torch.as_tensor(heads, device='cuda')
-        for k, r in runs.items():
-            same_layout = k[0] == configs[0][0]
-            g, g0 = r['grads'], first['grads']
-            assert torch.equal(g if same_layout else g[~heads], g0 if same_layout else g0[~heads]), \
-                (mode, k, 'gradients differ from', configs[0])
-            assert np.array_equal(r['h'], first['h']) and np.array_equal(r['c'], first['c']), (mode, k, 'states differ')
-        report.append('%s tc %.2e ffma %.2e' % (mode, worst_tc, max(r_ffma.values())))
-    print('[%s] B=%d T=%d N=%d worst per-entry ratio: %s' % (c['purpose'], B, T, N, '; '.join(report)))
+    e = _engine(lay, params, c, tc=True)
+    r = _run_unfused(e, lay, x, x['fp'], x['acts'], W) if mode == 'unfused' else _run_fused(e, lay, x, W)
+    del e
+    fp, acts = (x['fp'], x['acts']) if mode == 'unfused' else (r['fp'][:T], r['acts'])
+    ref = _oracle(lay, orc_args, params, c, x, n_s, fp, acts)
+    # calibration: the FP32-FFMA kernels on the same buffers against the same oracle
+    e = _engine(lay, params, c, tc=False)
+    ffma = _run_unfused(e, lay, x, fp, acts, W)
+    del e
+    r_ffma = _check('%s ffma' % mode, ffma, ref, used)
+    tag = '%s tc' % mode
+    r_tc = _check(tag, r, ref, used)
+    bad = {n: (r_tc[n], r_ffma[n]) for n in r_tc if r_tc[n] > 4 * r_ffma[n] + FLOOR}
+    assert not bad, (tag, 'per-entry error / round-off scale', sorted(bad.items(), key=lambda t: -t[1][0])[:6])
+    print('[%s] %s B=%d T=%d N=%d worst per-entry ratio: tc %.2e ffma %.2e' % (
+        c['purpose'], mode, B, T, N, max(r_tc.values()), max(r_ffma.values())))

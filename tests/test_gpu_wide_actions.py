@@ -55,9 +55,10 @@ TC += [pytest.param(dict(variant='ma2c_nc', B=256, T=8, topo='grid5', n_a=8, don
                          purpose='n_a = 11 with an agent without neighbours'), id='n_a11-cut-ma2c_dial')]
 
 
+@pytest.mark.parametrize('mode', ['unfused', 'fused'])
 @pytest.mark.parametrize('c', TC)
-def test_wide_tc_paths_match_fp64(c, monkeypatch):
-    test_gpu_tc_paths.test_tc_paths_match_fp64(c, monkeypatch)
+def test_wide_tc_paths_match_fp64(c, mode):
+    test_gpu_tc_paths.test_tc_paths_match_fp64(c, mode)
 
 
 @pytest.mark.parametrize('offset', [0, 3])

@@ -76,7 +76,7 @@ def main():
     t = np.array([update() for _ in range(args.updates)])
     e.check_tc()                                           # a timed-out pipeline wait would void the numbers
     print('card: %s' % card())
-    print('workload: %s, %d envs x %d agents, n_step %d, raw_tiles %d' % (args.config, e.B, e.N, e.T, int(e.raw_tiles)))
+    print('workload: %s, %d envs x %d agents, n_step %d' % (args.config, e.B, e.N, e.T))
     print('tc_wgrad_kernel in situ over %d eager updates: median %.1f us, min %.1f us, max %.1f us' %
           (len(t), np.median(t), t.min(), t.max()))
     if args.timeline:
