@@ -2,8 +2,8 @@
 
 Run in the authoring container only (needs the reference checkout, see make_golden.REF):
     python tests/golden/make_golden_wide_actions.py [--force]
-Writes tests/golden/wide_{ma2c_nc,ma2c_dial,ia2c_fp}.npz, tests/golden/wide_iso_ia2c_fp.npz and
-tests/golden/wide_n12_ma2c_nc.npz.  The fixtures are committed; nothing at test or bench time reads the reference.
+Writes tests/golden/wide_{ma2c_nc,ma2c_dial,ia2c_fp}.npz, tests/golden/wide_iso_ia2c_fp.npz,
+tests/golden/wide_n12_ma2c_nc.npz and tests/golden/wide_n12_h16_ma2c_nc.npz.  The fixtures are committed; nothing at test or bench time reads the reference.
 
   * wide_ma2c_nc / wide_ma2c_dial: make_golden.hetero_case on the HETERO graph.
   * wide_ia2c_fp: make_golden_hetero_ia2c.hetero_ia2c_case on the HETERO graph; wide_iso_ia2c_fp on the graph whose
@@ -12,6 +12,8 @@ tests/golden/wide_n12_ma2c_nc.npz.  The fixtures are committed; nothing at test 
     reference's `identical_agent` branch (agents/models.py:90-94, NCMultiAgentPolicy with lstm_comm) -- the
     homogeneous path the batched engine and the C ABI run.  make_golden.hetero_case refuses identical agents, so
     identical_case below drives the same scripted stream (same seeds, same recording) without that check.
+  * wide_n12_h16_ma2c_nc: wide_n12_ma2c_nc at num_lstm = num_fc = 16 (make_golden_hidden's width override), the
+    point where the narrow LSTM width meets the 16-wide head.  `n_h` records the width.
 The case functions are used unchanged; only the action counts they read are overridden: n_a_ls = N_A_LS, which mixes
 narrow agents with agents of 8 to 15 actions (the 16-wide head of the kernels).  The trained weights are kept as a
 W1_SAMPLE sample per tensor, as in the other heterogeneous fixtures.  Each case runs in a fresh process so that the
@@ -33,7 +35,8 @@ N_A_LS = [8, 3, 15, 2, 11, 6]
 N_A_SAME, N_S_SAME = 12, 5
 JOBS = [('wide_ma2c_nc', 'ma2c_nc', 'hetero'), ('wide_ma2c_dial', 'ma2c_dial', 'hetero'),
         ('wide_ia2c_fp', 'ia2c_fp', 'hetero'), ('wide_iso_ia2c_fp', 'ia2c_fp', 'hetero_iso_'),
-        ('wide_n12_ma2c_nc', 'ma2c_nc', 'same')]
+        ('wide_n12_ma2c_nc', 'ma2c_nc', 'same'), ('wide_n12_h16_ma2c_nc', 'ma2c_nc', 'same')]
+WIDTH = {'wide_n12_h16_ma2c_nc': 16}          # num_lstm = num_fc of the cases that override the config's 64
 
 
 def identical_case(agent, edges):
@@ -112,6 +115,9 @@ def identical_case(agent, edges):
 def run_case(job):
     name, agent, graph = job
     mg._import_reference()
+    if name in WIDTH:
+        import make_golden_hidden
+        make_golden_hidden._with_width(WIDTH[name])
     mg.HETERO['n_a_ls'] = list(N_A_LS)
     edges = mg.HETERO_ISO.get(graph, mg.HETERO['edges'])
     if graph == 'same':
@@ -121,6 +127,8 @@ def run_case(job):
     else:
         import make_golden_hetero_ia2c as mgi
         out = mgi.hetero_ia2c_case(agent, edges)
+    if name in WIDTH:
+        out['n_h'] = WIDTH[name]
     np.savez_compressed(os.path.join(HERE, name + '.npz'), **out)
     return name, out['trace'].shape, len(out['names'])
 

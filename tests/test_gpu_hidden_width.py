@@ -17,6 +17,7 @@
   n_h = 32 is ignored (same outputs as without it).
 """
 import configparser
+import contextlib
 import ctypes
 import hashlib
 import os
@@ -67,8 +68,10 @@ def _check_grads(tag, gk, orc):
         assert err <= 2e-5 * scale + 1e-7, (tag, n, err, scale)
 
 
-def _run_against_oracle(tag, eng, orc, lay, n_h, obs_o, base_dev, fp, acts, dones, Rs, Advs, advs_kernel=None):
-    """p / v forward of step 0, backward over T steps, gradients, padding and two optimizer steps."""
+def _run_against_oracle(tag, eng, orc, lay, n_h, obs_o, base_dev, fp, acts, dones, Rs, Advs, advs_kernel=None, judge=None):
+    """p / v forward of step 0, backward over T steps, gradients, padding and two optimizer steps.  `judge` replaces
+    the per-tensor gradient check: judge.mode(orc) is active around the oracle's backward, then
+    judge.check(tag, kernel gradients, orc) (tests/test_gpu_narrow_widths.py)."""
     T, B, N = acts.shape
     rs = np.random.RandomState(5)
     c0 = (rs.randn(B, N, n_h) * .5).astype(np.float32); h0 = (rs.rand(B, N, n_h) - .5).astype(np.float32)
@@ -95,8 +98,9 @@ def _run_against_oracle(tag, eng, orc, lay, n_h, obs_o, base_dev, fp, acts, done
     np.testing.assert_allclose(bn(v_d), v_o, rtol=0, atol=1e-5, err_msg=tag)
     # ---- backward ----
     orc.states_bw, orc.states_fw = st.clone(), st.clone()
-    summ = orc.backward(obs_o, fp.astype(np.float64), acts, dones, Rs, Advs, 5e-4, v_coef=HP['v_coef'],
-                        e_coef=HP['e_coef'], apply=False)
+    with judge.mode(orc) if judge else contextlib.nullcontext():
+        summ = orc.backward(obs_o, fp.astype(np.float64), acts, dones, Rs, Advs, 5e-4, v_coef=HP['v_coef'],
+                            e_coef=HP['e_coef'], apply=False)
     eng.T_cur = T
     eng.obs_buf[:T].copy_(base_dev)
     eng.fp_buf[:T].copy_(to_dev(np.transpose(fp, (0, 2, 1, 3))))
@@ -108,7 +112,7 @@ def _run_against_oracle(tag, eng, orc, lay, n_h, obs_o, base_dev, fp, acts, done
     eng.backward()
     torch.cuda.synchronize()
     flat = eng.grads.cpu().numpy()
-    _check_grads(tag, lay.unpack(flat), orc)
+    (judge.check if judge else _check_grads)(tag, lay.unpack(flat), orc)
     losses = eng.losses()
     for k in ('policy_loss', 'value_loss', 'entropy_loss'):        # per agent, the reference's weighting
         ref = np.asarray(summ[k], dtype=np.float64).ravel()

@@ -131,6 +131,13 @@ class RoundoffScale(TorchFunctionMode):
         self.sum_of = {}               # id(x @ W) -> id(x @ W + b)
         self.kink = {}                 # id(z) -> |gradient of relu(z)| on the rows where |z| < KINK, set in backward
 
+    def __exit__(self, *exc):
+        # the hooks hold this object, and the tensors in `keep` hold the hooks inside autograd's C++ graph: a cycle the
+        # Python collector cannot see, which would keep every hooked activation (and x) alive for good.  The backward
+        # has run inside the mode, so drop the tensors; S and K stay.
+        self.keep.clear(); self.sum_of.clear(); self.kink.clear()
+        return super().__exit__(*exc)
+
     def _acc(self, d, n, val):
         with torch.no_grad():
             d[n] += val
