@@ -53,6 +53,19 @@ class CaccCfg(C.Structure):
                                           'u_min', 'u_max', 'rew_a', 'rew_b', 'G')]
 
 
+ENV_PAR_FIELDS = ('h_star', 'v_star', 'h_s', 'h_g', 'v_max', 'u_min', 'u_max')   # nmarl_cacc_env_par order
+
+
+class CaccEnvPar(C.Structure):
+    """One row of the per-env scenario parameter table (the device table is [B] of these, 64 bytes each)."""
+    _fields_ = [(k, C.c_double) for k in ENV_PAR_FIELDS] + [('scenario', C.c_int32), ('pad_', C.c_int32)]
+
+
+class CaccParRanges(C.Structure):
+    _fields_ = [('lo', C.c_double * len(ENV_PAR_FIELDS)), ('hi', C.c_double * len(ENV_PAR_FIELDS)),
+                ('slowdown_prob', C.c_double)]
+
+
 class FwdArgs(C.Structure):
     _fields_ = [('B', C.c_int32), ('params', C.c_void_p), ('obs', C.c_void_p), ('fp', C.c_void_p),
                 ('done', C.c_void_p), ('c_in', C.c_void_p), ('h_in', C.c_void_p), ('msg_in', C.c_void_p),
@@ -82,7 +95,8 @@ class BwdArgs(C.Structure):
 _lib = None
 
 EXPORTS = ['nmarl_last_error', 'nmarl_version', 'nmarl_create', 'nmarl_destroy', 'nmarl_sizeof_bwd_args', 'nmarl_sizeof_fwd_args', 'nmarl_sizeof_model', 'nmarl_sizeof_agent', 'nmarl_sizeof_cacc_cfg',
-           'nmarl_cacc_reset', 'nmarl_cacc_step', 'nmarl_pack_weights', 'nmarl_policy_step_p', 'nmarl_policy_step_v', 'nmarl_dial_msg',
+           'nmarl_sizeof_cacc_env_par', 'nmarl_sizeof_cacc_par_ranges',
+           'nmarl_cacc_reset', 'nmarl_cacc_step', 'nmarl_cacc_reset_pe', 'nmarl_cacc_step_pe', 'nmarl_cacc_draw_par', 'nmarl_pack_weights', 'nmarl_policy_step_p', 'nmarl_policy_step_v', 'nmarl_dial_msg',
            'nmarl_rng_advance', 'nmarl_nstep_return_adv', 'nmarl_loss_tiles', 'nmarl_ws_floats', 'nmarl_operand_tile_offset',
            'nmarl_a2c_backward', 'nmarl_a2c_train_forward', 'nmarl_a2c_bptt',
            'nmarl_clip_rmsprop_step', 'nmarl_consensus_update', 'nmarl_eval_record']
@@ -104,6 +118,9 @@ def lib():
     L.nmarl_destroy.argtypes = [P]
     L.nmarl_cacc_reset.argtypes = [C.POINTER(CaccCfg), I, P, P, U64, P, P, P, P, P, P, P, P, I, P, I, P]
     L.nmarl_cacc_step.argtypes = [C.POINTER(CaccCfg), I, I, P, P, P, P, P, P, P, P, I, P, P, P, P]
+    L.nmarl_cacc_reset_pe.argtypes = [C.POINTER(CaccCfg), P, I, P, P, U64, P, P, P, P, P, P, P, P, I, P, I, P]
+    L.nmarl_cacc_step_pe.argtypes = [C.POINTER(CaccCfg), P, I, I, P, P, P, P, P, P, P, P, I, P, P, P, P]
+    L.nmarl_cacc_draw_par.argtypes = [C.POINTER(CaccCfg), C.POINTER(CaccParRanges), I, U64, P, P, P, P]
     L.nmarl_policy_step_p.argtypes = [C.POINTER(Model), C.POINTER(FwdArgs), P]
     L.nmarl_policy_step_v.argtypes = [C.POINTER(Model), C.POINTER(FwdArgs), P]
     L.nmarl_dial_msg.argtypes = [C.POINTER(Model), I, P, P, P, P]
@@ -122,6 +139,8 @@ def lib():
     assert L.nmarl_sizeof_model() == C.sizeof(Model), 'nmarl_model layout mismatch'
     assert L.nmarl_sizeof_agent() == C.sizeof(Agent), 'nmarl_agent layout mismatch'
     assert L.nmarl_sizeof_cacc_cfg() == C.sizeof(CaccCfg), 'nmarl_cacc_cfg layout mismatch'
+    assert L.nmarl_sizeof_cacc_env_par() == C.sizeof(CaccEnvPar), 'nmarl_cacc_env_par layout mismatch'
+    assert L.nmarl_sizeof_cacc_par_ranges() == C.sizeof(CaccParRanges), 'nmarl_cacc_par_ranges layout mismatch'
     assert L.nmarl_sizeof_bwd_args() == C.sizeof(BwdArgs), 'nmarl_bwd_args layout mismatch'
     assert L.nmarl_sizeof_fwd_args() == C.sizeof(FwdArgs), 'nmarl_fwd_args layout mismatch'
     _lib = L

@@ -16,11 +16,14 @@ extern "C" const char* nmarl_last_error(void) { return g_err; }
 // 101: NMARL_MAX_AGENT 32 -> 128; 102: n_h = 16 / 32 (s_dim); 103: nmarl_eval_record; 104: n_a up to 15 (sv_dlv rows
 // are nmarl_head_width(n_a) floats wide); 105: nmarl_a2c_bptt always computes the heads; the bwd_args field and the
 // entry point that chose whether it did are gone; 106: nmarl_bwd_args.raw_tiles is gone (sv_dzT / sv_dpT always hold
-// one raw tile per 32 rows, half the size), and state_fm must match the layout the path runs
-extern "C" int nmarl_version(void) { return 106; }
+// one raw tile per 32 rows, half the size), and state_fm must match the layout the path runs; 107: per-env scenario
+// parameters (nmarl_cacc_env_par, nmarl_cacc_draw_par, nmarl_cacc_reset_pe / nmarl_cacc_step_pe)
+extern "C" int nmarl_version(void) { return 107; }
 extern "C" int nmarl_sizeof_model(void) { return (int)sizeof(nmarl_model); }
 extern "C" int nmarl_sizeof_agent(void) { return (int)sizeof(nmarl_agent); }
 extern "C" int nmarl_sizeof_cacc_cfg(void) { return (int)sizeof(nmarl_cacc_cfg); }
+extern "C" int nmarl_sizeof_cacc_env_par(void) { return (int)sizeof(nmarl_cacc_env_par); }
+extern "C" int nmarl_sizeof_cacc_par_ranges(void) { return (int)sizeof(nmarl_cacc_par_ranges); }
 extern "C" int nmarl_sizeof_fwd_args(void) { return (int)sizeof(nmarl_fwd_args); }
 extern "C" int nmarl_sizeof_bwd_args(void) { return (int)sizeof(nmarl_bwd_args); }
 extern "C" int64_t nmarl_operand_tile_offset(int rows, int t, int n_agent, int B, int agent, int block) {

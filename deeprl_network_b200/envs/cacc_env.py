@@ -12,7 +12,12 @@ New optional keys in ``ENV_CONFIG`` (everything else parses exactly like the ref
   platoon_len  vehicles per platoon (default n_vehicle); < n_vehicle gives several independent
                platoons -- used only by the synthetic 5x5-grid configuration
   topology     'chain' (default) or 'grid' (row-major 4-neighbour grid, Manhattan distance)
+Per-env scenario parameters (batched training only, n_env > 1; all absent by default -- see ``parse_env_par``):
+  <key>_range  = lo, hi  for headway_target, speed_target, headway_st, headway_go, speed_max, accel_min, accel_max:
+               each env draws its own value from U[lo, hi) whenever it resets
+  slowdown_prob = p      each env runs slow-down with probability p, else catch-up (default: `scenario` for all)
 """
+import configparser
 import ctypes as C
 import logging
 
@@ -40,18 +45,93 @@ def grid_masks(side):
     return (dist == 1).astype(int), dist
 
 
+# ENV_CONFIG key -> field of the per-env parameter table (nmarl_cacc_env_par), in table order
+PAR_KEYS = dict(zip(('headway_target', 'speed_target', 'headway_st', 'headway_go', 'speed_max', 'accel_min',
+                     'accel_max'), L.ENV_PAR_FIELDS))
+ENV_PAR_KEYS = tuple(k + '_range' for k in PAR_KEYS) + ('slowdown_prob',)
+
+
+def env_par_keys(config):
+    """The per-env parameter keys present in an ENV_CONFIG section."""
+    return [k for k in ENV_PAR_KEYS if k in config]
+
+
+def nominal_config(config):
+    """A copy of an ENV_CONFIG section without the per-env parameter keys: every env runs the config's nominal
+    values.  Evaluation uses it, so that test rewards stay comparable across runs."""
+    cp = configparser.ConfigParser(interpolation=None)
+    cp.read_dict({'ENV_CONFIG': {k: config.get(k, raw=True) for k in config if k not in ENV_PAR_KEYS}})
+    return cp['ENV_CONFIG']
+
+
+def parse_env_par(config, h_min=None):
+    """ENV_CONFIG section -> the draw ranges of the per-env parameter table, or None when no key is present.
+
+    Returns {'ranges': {field: (lo, hi)} for every field of L.ENV_PAR_FIELDS (a field without its key gets the
+    point range of its nominal value), 'slowdown_prob': p or None}.  Raises ValueError, naming the key, unless
+    lo <= hi for every range and every draw keeps headway_min < headway_st < headway_go, accel_min < 0 < accel_max,
+    speed_target > 0 and headway_target > 0, and 0 <= slowdown_prob <= 1 (the checks nmarl_cacc_draw_par repeats)."""
+    if not env_par_keys(config):
+        return None
+    h_min = config.getfloat('headway_min') if h_min is None else h_min
+    ranges = {}
+    for key, field in PAR_KEYS.items():
+        if key + '_range' not in config:
+            v = config.getfloat(key)
+            ranges[field] = (v, v)
+            continue
+        txt = config.get(key + '_range')
+        try:
+            lo, hi = (float(x) for x in txt.split(','))
+        except ValueError:
+            raise ValueError('ENV_CONFIG.%s_range = %r: expected two numbers "lo, hi"' % (key, txt)) from None
+        if not lo <= hi:
+            raise ValueError('ENV_CONFIG.%s_range = %r: needs lo <= hi' % (key, txt))
+        ranges[field] = (lo, hi)
+    lo = {f: r[0] for f, r in ranges.items()}
+    hi = {f: r[1] for f, r in ranges.items()}
+    if not h_min < lo['h_s']:
+        raise ValueError('headway_st (from %g) must exceed headway_min (%g) for every draw' % (lo['h_s'], h_min))
+    if not hi['h_s'] < lo['h_g']:
+        raise ValueError('headway_st (up to %g) must stay below headway_go (from %g) for every draw'
+                         % (hi['h_s'], lo['h_g']))
+    if not hi['u_min'] < 0:
+        raise ValueError('accel_min (up to %g) must be negative for every draw' % hi['u_min'])
+    if not lo['u_max'] > 0:
+        raise ValueError('accel_max (from %g) must be positive for every draw' % lo['u_max'])
+    if not lo['v_star'] > 0:
+        raise ValueError('speed_target (from %g) must be positive for every draw' % lo['v_star'])
+    if not lo['h_star'] > 0:
+        raise ValueError('headway_target (from %g) must be positive for every draw' % lo['h_star'])
+    p = None
+    if 'slowdown_prob' in config:
+        p = config.getfloat('slowdown_prob')
+        if not 0 <= p <= 1:
+            raise ValueError('ENV_CONFIG.slowdown_prob = %g: needs 0 <= p <= 1' % p)
+    return {'ranges': ranges, 'slowdown_prob': p}
+
+
 class CACCEnv:
     def __init__(self, config, n_env=None, device=None):
         L.require_cuda()
         self._load_config(config)
         if n_env is not None:
             self.n_env = int(n_env)
+        if self.par_spec is not None and self.n_env == 1:
+            raise ValueError('ENV_CONFIG keys %s (per-env scenario parameters) need batched training: set n_env > 1 '
+                             '(VecTrainer); the one-env Trainer runs the nominal values only'
+                             % ', '.join(env_par_keys(config)))
         self.device = torch.device(device if device is not None else 'cuda:%d' % torch.cuda.current_device())
         self.train_mode = True
         self.cur_episode = 0
         self.is_record = False
         self._init_space()
         self._alloc()
+        if self.par_spec is not None:
+            sp = self.par_spec
+            logging.info('per-env scenario parameters, redrawn at every reset: %s; %s' % (
+                ', '.join('%s in [%g, %g]' % (k, *sp['ranges'][f]) for k, f in PAR_KEYS.items()),
+                'scenario %s' % self.name if sp['slowdown_prob'] is None else 'slowdown_prob %g' % sp['slowdown_prob']))
         # "required to achieve the same model initialization" (envs/cacc_env.py:21-22)
         np.random.seed(self.seed)
 
@@ -84,6 +164,7 @@ class CACCEnv:
         self.topology = config.get('topology', fallback='chain')
         if not (self.name.startswith('catchup') or self.name.startswith('slowdown')):
             raise ValueError('unknown CACC scenario %r' % self.name)
+        self.par_spec = parse_env_par(config, self.h_min)
 
     def _init_space(self):
         if self.topology == 'grid':
@@ -128,6 +209,16 @@ class CACCEnv:
         c.v_max, c.v_star, c.u_min, c.u_max = self.v_max, self.v_star, self.u_min, self.u_max
         c.rew_a, c.rew_b, c.G = self.a, self.b, self.G
         self.cfg = c
+        # per-env scenario parameters: [B] rows of nmarl_cacc_env_par (8 x 8 bytes; the last holds the int32 scenario)
+        self.env_par = None
+        if self.par_spec is not None:
+            self.env_par = torch.zeros(B, C.sizeof(L.CaccEnvPar) // 8, **f64)
+            r = L.CaccParRanges()
+            for k, f in enumerate(L.ENV_PAR_FIELDS):
+                r.lo[k], r.hi[k] = self.par_spec['ranges'][f]
+            p = self.par_spec['slowdown_prob']
+            r.slowdown_prob = -1.0 if p is None else p
+            self._par_ranges = r
         self.collision = False
         self.t = 0
 
@@ -138,6 +229,17 @@ class CACCEnv:
         obs = self.obs_dev if obs_out is None else obs_out
         fp = self.fp_dev if fp_out is None else fp_out
         seed = int(self.cfg_seed if philox_seed is None else philox_seed) & (2 ** 64 - 1)
+        if self.env_par is not None:
+            # the reset envs draw their parameters for the episode they start (Philox keyed by seed, env, episode)
+            L.check(L.lib().nmarl_cacc_draw_par(C.byref(self.cfg), C.byref(self._par_ranges), self.n_env, seed,
+                                                L.ptr(self.episode_dev), L.ptr(mask), L.ptr(self.env_par),
+                                                L.stream()), 'nmarl_cacc_draw_par')
+            L.check(L.lib().nmarl_cacc_reset_pe(C.byref(self.cfg), L.ptr(self.env_par), self.n_env, L.ptr(u01),
+                                                L.ptr(mask), seed, L.ptr(self.episode_dev), L.ptr(self.hs),
+                                                L.ptr(self.vs), L.ptr(self.us), L.ptr(self.t_dev),
+                                                L.ptr(self.collision_dev), L.ptr(self.v_init), L.ptr(obs),
+                                                obs.shape[-1], L.ptr(fp), self.n_a, L.stream()), 'nmarl_cacc_reset_pe')
+            return
         L.check(L.lib().nmarl_cacc_reset(C.byref(self.cfg), self.n_env, L.ptr(u01), L.ptr(mask), seed,
                                          L.ptr(self.episode_dev), L.ptr(self.hs), L.ptr(self.vs), L.ptr(self.us),
                                          L.ptr(self.t_dev), L.ptr(self.collision_dev), L.ptr(self.v_init),
@@ -149,6 +251,13 @@ class CACCEnv:
         rew = self.reward_dev if reward_out is None else reward_out
         grew = self.greward_dev if greward_out is None else greward_out
         done = self.done_dev if done_out is None else done_out
+        if self.env_par is not None:
+            L.check(L.lib().nmarl_cacc_step_pe(C.byref(self.cfg), L.ptr(self.env_par), self.n_env, int(self.train_mode),
+                                               L.ptr(action), L.ptr(self.hs), L.ptr(self.vs), L.ptr(self.us),
+                                               L.ptr(self.t_dev), L.ptr(self.collision_dev), L.ptr(self.v_init),
+                                               L.ptr(obs), obs.shape[-1], L.ptr(rew), L.ptr(grew), L.ptr(done),
+                                               L.stream()), 'nmarl_cacc_step_pe')
+            return
         L.check(L.lib().nmarl_cacc_step(C.byref(self.cfg), self.n_env, int(self.train_mode), L.ptr(action),
                                         L.ptr(self.hs), L.ptr(self.vs), L.ptr(self.us), L.ptr(self.t_dev),
                                         L.ptr(self.collision_dev), L.ptr(self.v_init), L.ptr(obs), obs.shape[-1],
@@ -157,6 +266,23 @@ class CACCEnv:
     @property
     def cfg_seed(self):
         return getattr(self, '_cfg_seed', 0)
+
+    def par_table(self):
+        """Host copy of the per-env parameter table: {field: float64 [B]} and 'scenario': int32 [B].  Host sync."""
+        t = self.env_par.cpu()
+        out = {f: t[:, k].numpy() for k, f in enumerate(L.ENV_PAR_FIELDS)}
+        out['scenario'] = t.view(torch.int32)[:, 2 * len(L.ENV_PAR_FIELDS)].numpy()
+        return out
+
+    def par_stats(self):
+        """Mean, min and max over the batch of every drawn field (and of `slowdown`: 1 for a slow-down env), as one
+        flat record {<field>_mean, <field>_min, <field>_max}.  Host sync."""
+        tab = self.par_table()
+        tab['slowdown'] = (tab.pop('scenario') == L.SLOWDOWN).astype(np.float64)
+        rec = {}
+        for f, v in tab.items():
+            rec.update({f + '_mean': float(v.mean()), f + '_min': float(v.min()), f + '_max': float(v.max())})
+        return rec
 
     # ---- reference API (host arrays, env 0 is "the" environment) -----------------------------------
     def _host_obs(self):

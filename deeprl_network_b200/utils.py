@@ -22,7 +22,7 @@ import torch
 
 from . import _lib as L
 from .agents.engine import PolicyEngine
-from .envs.cacc_env import CACCEnv, control_record, traffic_frame, write_records
+from .envs.cacc_env import CACCEnv, control_record, env_par_keys, nominal_config, traffic_frame, write_records
 from .layout import ModelLayout
 
 _TEST_MODES = {'no_test': (False, False), 'in_train_test': (True, False),
@@ -136,6 +136,9 @@ class Trainer:
     actions come from ``np.random.choice`` like in the reference."""
 
     def __init__(self, env, model, global_counter, summary_writer, output_path=None, uniform_fn=None):
+        if getattr(env, 'env_par', None) is not None:
+            raise ValueError('per-env scenario parameters (ENV_CONFIG *_range / slowdown_prob) need batched training '
+                             '(VecTrainer, n_env > 1)')
         self.env, self.model, self.global_counter = env, model, global_counter
         self.summary_writer, self.output_path, self.uniform_fn = summary_writer, output_path, uniform_fn
         self.agent = env.agent
@@ -295,6 +298,7 @@ class VecTrainer:
             raise AssertionError('VecTrainer: episode length %d / env batch_size %d are not multiples of the update '
                                  'length %d' % (env.T, env.batch_size, model.n_step))
         self.data = []                     # one record per update (train_reward.csv of the batched loop)
+        self.par_data = []                 # with per-env scenario parameters: env_par.csv, one row per log record
 
     def start(self):
         self._seed = self.env.seed
@@ -347,13 +351,19 @@ class VecTrainer:
         g = self.engine.grew_buf[:self.engine.T_cur]
         mean, std = float(g.mean().item()), float(g.std(unbiased=False).item())
         self.data.append(dict(agent=self.env.agent, step=int(global_step), test_id=-1, avg_reward=mean, std_reward=std))
+        if getattr(self.env, 'env_par', None) is not None:
+            self.par_data.append(dict(step=int(global_step), **self.env.par_stats()))
         if summary_writer is not None:
             summary_writer.add_scalar('train_reward', mean, int(global_step))
         return mean
 
     def write_csv(self, output_path):
+        """train_reward.csv and, with per-env scenario parameters, env_par.csv: per log record the mean / min / max over
+        the batch of every drawn field (the table as it stands at the record: the parameters of the running episodes)."""
         import pandas as pd
         pd.DataFrame(self.data).to_csv(output_path + 'train_reward.csv')
+        if self.par_data:
+            pd.DataFrame(self.par_data).to_csv(output_path + 'env_par.csv')
 
 
 class BatchedEvaluator:
@@ -372,9 +382,14 @@ class BatchedEvaluator:
     Seeds go through in passes of at most ``max_env`` envs whose records fit in ``record_bytes`` of device memory
     (DESIGN §4.7).  With ``graph`` the steps of a pass are captured into a CUDA graph on the second pass of a size
     and replayed from then on.
+
+    Evaluation always runs the config's nominal scenario parameters: per-env parameter keys (``*_range``,
+    ``slowdown_prob``) of a training config are ignored here, so test rewards stay comparable across runs.
     """
 
     def __init__(self, env_config, model, output_path=None, max_env=4096, record_bytes=2 ** 31, graph=True):
+        if env_par_keys(env_config):
+            env_config = nominal_config(env_config)
         self.config, self.model, self.output_path = env_config, model, output_path
         self.max_env, self.record_bytes, self.use_graph = int(max_env), int(record_bytes), graph
         self.layout = self._eval_layout(model.layout)

@@ -100,6 +100,24 @@ typedef struct {
   double dt, h_min, h_star, h_s, h_g, v_max, v_star, u_min, u_max, rew_a, rew_b, G;
 } nmarl_cacc_cfg;
 
+/* ---- per-env CACC scenario parameters (table [B], one row per env) ----------------------------
+ * Read by nmarl_cacc_reset_pe / nmarl_cacc_step_pe in place of the same-named fields of nmarl_cacc_cfg; every
+ * other field (dt, h_min, T, batch_size, reward weights, ...) stays the config's.                     */
+typedef struct {
+  double h_star, v_star, h_s, h_g, v_max, u_min, u_max;
+  int32_t scenario;                      /* NMARL_CATCHUP / NMARL_SLOWDOWN                      */
+  int32_t pad_;
+} nmarl_cacc_env_par;
+
+/* Ranges nmarl_cacc_draw_par draws the table from: field k of a row (nmarl_cacc_env_par order, k < 7) is
+ * lo[k] + u * (hi[k] - lo[k]); lo[k] == hi[k] gives exactly lo[k].  slowdown_prob < 0: every env runs
+ * cfg->scenario; in [0, 1]: an env runs slow-down with this probability, else catch-up.             */
+#define NMARL_ENV_PAR_FIELDS 7
+typedef struct {
+  double lo[NMARL_ENV_PAR_FIELDS], hi[NMARL_ENV_PAR_FIELDS];
+  double slowdown_prob;
+} nmarl_cacc_par_ranges;
+
 const char* nmarl_last_error(void);
 int nmarl_version(void);
 /* ---- context (SURVEY 8b): owns the helper stream/events of the CURRENT device; no other state ---------- */
@@ -110,6 +128,8 @@ int nmarl_destroy(nmarl_ctx* ctx);
 int nmarl_sizeof_model(void);
 int nmarl_sizeof_agent(void);
 int nmarl_sizeof_cacc_cfg(void);
+int nmarl_sizeof_cacc_env_par(void);
+int nmarl_sizeof_cacc_par_ranges(void);
 int nmarl_sizeof_fwd_args(void);
 int nmarl_sizeof_bwd_args(void);
 
@@ -132,6 +152,26 @@ int nmarl_cacc_reset(const nmarl_cacc_cfg* cfg, int B, const double* u01, const 
 int nmarl_cacc_step(const nmarl_cacc_cfg* cfg, int B, int train_mode, const int32_t* action,
                     double* hs, double* vs, double* us, int32_t* t, int32_t* collision, const double* v_init,
                     float* obs, int obs_stride, double* reward, double* greward, float* done, void* stream);
+/* The same two calls with per-env scenario parameters: env b reads h_star, v_star, h_s, h_g, v_max, u_min, u_max and
+ * scenario from par[b] (device nmarl_cacc_env_par [B]) and behaves exactly like the one-env CACCEnv constructed
+ * with those values.  Every other argument is that of nmarl_cacc_reset / nmarl_cacc_step.                      */
+int nmarl_cacc_reset_pe(const nmarl_cacc_cfg* cfg, const nmarl_cacc_env_par* par, int B, const double* u01,
+                        const float* mask, uint64_t seed, int32_t* episode,
+                        double* hs, double* vs, double* us, int32_t* t, int32_t* collision, double* v_init,
+                        float* obs, int obs_stride, float* fp, int n_a, void* stream);
+int nmarl_cacc_step_pe(const nmarl_cacc_cfg* cfg, const nmarl_cacc_env_par* par, int B, int train_mode,
+                       const int32_t* action, double* hs, double* vs, double* us, int32_t* t, int32_t* collision,
+                       const double* v_init, float* obs, int obs_stride, double* reward, double* greward,
+                       float* done, void* stream);
+/* Draw the table rows of the envs with mask[b] != 0 (mask NULL: all) for the episode they are about to start:
+ * call it before nmarl_cacc_reset_pe with the same seed, episode and mask (episode NULL: counter 0).
+ * Keying: Philox4x32-10, key = (seed low, seed high), counter words = (c low, c high, env, 0x454e5650) with
+ * c = episode[b] << 8 | k; u = ((w0 >> 5) * 2^26 + (w1 >> 6)) / 2^53 from output words 0, 1.  k = 0..6 draw the
+ * fields in nmarl_cacc_env_par order, k = 7 the scenario (slow-down iff u < slowdown_prob).
+ * Checked before the launch, with a message each: lo <= hi for every field; cfg->h_min < h_s and h_s < h_g for
+ * every draw (h_min < lo[h_s], hi[h_s] < lo[h_g]); u_min < 0 < u_max; v_star > 0; h_star > 0; slowdown_prob <= 1. */
+int nmarl_cacc_draw_par(const nmarl_cacc_cfg* cfg, const nmarl_cacc_par_ranges* ranges, int B, uint64_t seed,
+                        const int32_t* episode, const float* mask, nmarl_cacc_env_par* par, void* stream);
 
 /* ---- K2-K6: fused message-gather + encoders + LSTM cell + heads ----------------------------
  * Replaces lstm / lstm_comm / lstm_ic3 / lstm_dial (agents/utils.py:87-115,118-217,344-417,
@@ -162,7 +202,9 @@ typedef struct {
                            /* output words 0, 1.  The call does not move rng[1]: a rollout      */
                            /* passes offsets 0..T and then calls nmarl_rng_advance(rng, T + 1). */
                            /* nmarl_cacc_reset draws from the same generator with counter =     */
-                           /* episode << 8 | platoon, lane = env and the tag 0x454e5601         */
+                           /* episode << 8 | platoon, lane = env and the tag 0x454e5601, and    */
+                           /* nmarl_cacc_draw_par with counter = episode << 8 | parameter k,     */
+                           /* lane = env and the tag 0x454e5650                                  */
   const int32_t* act_in;   /* v-call: [N][B] same-step actions                                 */
   float* v;                /* v-call: [N][B]                                                   */
   const float* wpack;      /* packed 3xTF32 operands (nmarl_pack_weights) or NULL.  When set and  */

@@ -8,7 +8,9 @@ The reference's command line is kept verbatim (main.py:21-40 there) so existing 
 and so is the .ini surface (MODEL_CONFIG / TRAIN_CONFIG / ENV_CONFIG).  Optional new keys: ENV_CONFIG.n_env
 (parallel episodes per process) and TRAIN_CONFIG.greedy_test (default false).  n_env = 1 runs the reference's
 one-episode-at-a-time Trainer; n_env > 1 the device-resident VecTrainer, which with greedy_test also logs the greedy
-test reward over ENV_CONFIG.test_seeds to data/test_reward.csv.  evaluate runs all seeds at once on the device and
+test reward over ENV_CONFIG.test_seeds to data/test_reward.csv.  With n_env > 1, ENV_CONFIG.<key>_range / slowdown_prob
+give every env its own scenario parameters, redrawn at each of its resets (data/env_par.csv records what was drawn);
+evaluation keeps the nominal values.  evaluate runs all seeds at once on the device and
 writes the files the reference's one-seed-at-a-time Evaluator writes.  Agents: ia2c, ia2c_fp, ma2c_cu, ma2c_nc, ma2c_ic3, ma2c_dial on the CACC scenarios;
 ATSC/SUMO environments are out of scope (SURVEY row 10).
 """
@@ -18,7 +20,7 @@ import logging
 import os
 
 from deeprl_network_b200.agents import models as agent_models
-from deeprl_network_b200.envs.cacc_env import CACCEnv
+from deeprl_network_b200.envs.cacc_env import CACCEnv, nominal_config
 from deeprl_network_b200 import utils as U
 
 AGENTS = {'ia2c': agent_models.IA2C, 'ia2c_fp': agent_models.IA2C_FP, 'ma2c_cu': agent_models.IA2C_CU,
@@ -126,8 +128,9 @@ def evaluate_fn(agent_dir, output_dir, seeds, port, demo):
     if not ini:
         return
     cfg = read_config(ini)
-    cfg['ENV_CONFIG']['n_env'] = '1'
-    env = init_env(cfg['ENV_CONFIG'], port=port)
+    env_cfg = nominal_config(cfg['ENV_CONFIG'])          # evaluation runs the nominal scenario parameters
+    env_cfg['n_env'] = '1'
+    env = init_env(env_cfg, port=port)
     env.init_test_seeds(seeds)
     model = init_agent(env, cfg['MODEL_CONFIG'], 0, 0)
     if model is None or not model.load(agent_dir + '/model/'):
@@ -136,7 +139,7 @@ def evaluate_fn(agent_dir, output_dir, seeds, port, demo):
         # --demo writes no files; agents without a device engine run the seeds one at a time
         U.Evaluator(env, model, output_dir, gui=demo).run()
     else:
-        U.BatchedEvaluator(cfg['ENV_CONFIG'], model, output_dir).run(seeds)
+        U.BatchedEvaluator(env_cfg, model, output_dir).run(seeds)
 
 
 def evaluate(args):
