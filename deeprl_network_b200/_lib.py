@@ -74,7 +74,7 @@ class FwdArgs(C.Structure):
                 ('uniforms', C.c_void_p), ('rng', C.c_void_p), ('rng_offset', C.c_uint64),
                 ('act_in', C.c_void_p), ('v', C.c_void_p), ('wpack', C.c_void_p), ('tc_err', C.c_void_p),
                 ('sv_xin', C.c_void_p), ('sv_sh', C.c_void_p), ('sv_gates', C.c_void_p), ('sv_enc', C.c_void_p),
-                ('state_fm', C.c_int32)]
+                ('state_fm', C.c_int32), ('env0', C.c_int32), ('B_total', C.c_int32)]
 
 
 class BwdArgs(C.Structure):
@@ -96,7 +96,8 @@ _lib = None
 
 EXPORTS = ['nmarl_last_error', 'nmarl_version', 'nmarl_create', 'nmarl_destroy', 'nmarl_sizeof_bwd_args', 'nmarl_sizeof_fwd_args', 'nmarl_sizeof_model', 'nmarl_sizeof_agent', 'nmarl_sizeof_cacc_cfg',
            'nmarl_sizeof_cacc_env_par', 'nmarl_sizeof_cacc_par_ranges',
-           'nmarl_cacc_reset', 'nmarl_cacc_step', 'nmarl_cacc_reset_pe', 'nmarl_cacc_step_pe', 'nmarl_cacc_draw_par', 'nmarl_pack_weights', 'nmarl_policy_step_p', 'nmarl_policy_step_v', 'nmarl_dial_msg',
+           'nmarl_cacc_reset', 'nmarl_cacc_step', 'nmarl_cacc_reset_pe', 'nmarl_cacc_step_pe', 'nmarl_cacc_draw_par',
+           'nmarl_cacc_reset_shard', 'nmarl_cacc_reset_pe_shard', 'nmarl_cacc_draw_par_shard', 'nmarl_pack_weights', 'nmarl_policy_step_p', 'nmarl_policy_step_v', 'nmarl_dial_msg',
            'nmarl_rng_advance', 'nmarl_nstep_return_adv', 'nmarl_loss_tiles', 'nmarl_ws_floats', 'nmarl_operand_tile_offset',
            'nmarl_a2c_backward', 'nmarl_a2c_train_forward', 'nmarl_a2c_bptt',
            'nmarl_clip_rmsprop_step', 'nmarl_consensus_update', 'nmarl_eval_record']
@@ -121,6 +122,9 @@ def lib():
     L.nmarl_cacc_reset_pe.argtypes = [C.POINTER(CaccCfg), P, I, P, P, U64, P, P, P, P, P, P, P, P, I, P, I, P]
     L.nmarl_cacc_step_pe.argtypes = [C.POINTER(CaccCfg), P, I, I, P, P, P, P, P, P, P, P, I, P, P, P, P]
     L.nmarl_cacc_draw_par.argtypes = [C.POINTER(CaccCfg), C.POINTER(CaccParRanges), I, U64, P, P, P, P]
+    L.nmarl_cacc_reset_shard.argtypes = L.nmarl_cacc_reset.argtypes + [I]
+    L.nmarl_cacc_reset_pe_shard.argtypes = L.nmarl_cacc_reset_pe.argtypes + [I]
+    L.nmarl_cacc_draw_par_shard.argtypes = L.nmarl_cacc_draw_par.argtypes + [I]
     L.nmarl_policy_step_p.argtypes = [C.POINTER(Model), C.POINTER(FwdArgs), P]
     L.nmarl_policy_step_v.argtypes = [C.POINTER(Model), C.POINTER(FwdArgs), P]
     L.nmarl_dial_msg.argtypes = [C.POINTER(Model), I, P, P, P, P]

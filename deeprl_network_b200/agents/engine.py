@@ -34,12 +34,16 @@ def operand_tile_shapes(variant, N, B, T, n_h):
 
 class PolicyEngine:
     def __init__(self, layout, n_env, n_step, hp, flat_params=None, device=None, rng_seed=0,
-                 distance_mask=None, coop_gamma=-1.0, group=None, use_tc=None, shared_params=None):
+                 distance_mask=None, coop_gamma=-1.0, group=None, use_tc=None, shared_params=None, env0=0,
+                 n_env_total=None):
         """hp: dict(v_coef, e_coef, max_grad_norm, alpha, epsilon, gamma, reward_norm, reward_clip).
         shared_params: another engine's parameter tensor, read in place instead of a copy of flat_params (an
-        evaluation engine that follows the trained weights; it must not be trained itself)."""
+        evaluation engine that follows the trained weights; it must not be trained itself).
+        env0 / n_env_total: this engine's n_env envs are the global envs env0 .. env0 + n_env - 1 of a run sharded
+        over processes; the sampled actions are keyed by the global env index (nmarl_fwd_args.env0 / B_total)."""
         L.require_cuda()
         self.layout, self.B, self.T, self.hp = layout, int(n_env), int(n_step), dict(hp)
+        self.env0, self.B_glob = int(env0), self.B if n_env_total is None else int(n_env_total)
         self.N, self.n_a, self.n_h = layout.N, layout.n_a, layout.n_h
         self.device = torch.device(device if device is not None else 'cuda:%d' % torch.cuda.current_device())
         self.group = group
@@ -193,6 +197,7 @@ class PolicyEngine:
         a.params, a.obs, a.fp, a.done = L.ptr(self.params), L.ptr(obs), L.ptr(fp), L.ptr(done)
         a.c_in, a.h_in, a.msg_in = L.ptr(self.c[self.cur]), L.ptr(self.h[self.cur]), L.ptr(self.msg[self.cur])
         a.wpack, a.tc_err, a.state_fm = L.ptr(self.wpack), L.ptr(self.tc_err), int(self.state_fm)
+        a.env0, a.B_total = self.env0, self.B_glob
         return a
 
     def step_p(self, obs, fp, done, pi_out, action_out=None, sample_mode=L.SAMPLE_NONE, uniforms=None, rng_offset=0):
@@ -257,6 +262,7 @@ class PolicyEngine:
         a.B = self.B
         a.params, a.obs, a.fp, a.done = L.ptr(self.params), L.ptr(obs), L.ptr(fp), L.ptr(done)
         a.wpack, a.tc_err, a.state_fm = L.ptr(self.wpack), L.ptr(self.tc_err), int(self.state_fm)
+        a.env0, a.B_total = self.env0, self.B_glob
         ms = self.msg_seq
         if which == 'p':
             a.c_in, a.h_in, a.msg_in = L.ptr(self.c_seq[t]), L.ptr(self.h_seq[t]), L.ptr(None if ms is None else ms[t])

@@ -7,7 +7,9 @@ out, so ``Trainer`` and ``main.py`` run unchanged.  Underneath, everything is ex
 libnmarl CUDA kernels through :class:`PolicyEngine`; there is no TF session (``sess`` is None).
 
 Extra keyword arguments (not in the reference): ``n_env`` parallel environments (default 1,
-which is exactly the reference), ``device``, ``obs_mode`` (IA2C only, see ModelLayout).
+which is exactly the reference), ``device``, ``obs_mode`` (IA2C only, see ModelLayout), and for one shard of a
+run over several processes ``env0`` / ``n_env_total`` (the global index of this shard's first env, the run's env
+count: the sampled actions are keyed by the global env index).
 With ``n_env > 1`` use the batched entry points ``rollout`` / ``update`` (device resident).
 """
 import logging
@@ -27,14 +29,15 @@ class IA2C:
     variant = 'ia2c'
 
     def __init__(self, n_s_ls, n_a_ls, neighbor_mask, distance_mask, coop_gamma,
-                 total_step, model_config, seed=0, n_env=1, device=None, obs_mode=None, flat_params=None):
+                 total_step, model_config, seed=0, n_env=1, device=None, obs_mode=None, flat_params=None, env0=0,
+                 n_env_total=None):
         self.name = self.variant
         self._init_algo(n_s_ls, n_a_ls, neighbor_mask, distance_mask, coop_gamma, total_step, seed,
-                        model_config, n_env, device, obs_mode, flat_params)
+                        model_config, n_env, device, obs_mode, flat_params, env0, n_env_total)
 
     # ---- construction (agents/models.py:84-158, 246-258) ------------------------------------------
     def _init_algo(self, n_s_ls, n_a_ls, neighbor_mask, distance_mask, coop_gamma, total_step, seed,
-                   model_config, n_env, device, obs_mode, flat_params):
+                   model_config, n_env, device, obs_mode, flat_params, env0=0, n_env_total=None):
         self.n_s_ls, self.n_a_ls = list(n_s_ls), list(n_a_ls)
         # agents/models.py:89-97: agents are "identical" iff all action spaces are equal; otherwise inputs are
         # zero-padded to the widest agent and the *_hetero layers slice each agent's valid part
@@ -85,7 +88,8 @@ class IA2C:
                       epsilon=model_config.getfloat('rmsp_epsilon'), gamma=model_config.getfloat('gamma'))
         # weights come from the global NumPy stream in the reference's variable-creation order
         self.engine = PolicyEngine(self.layout, self.n_env, self.n_step, hp, flat_params=flat_params, device=device,
-                                   rng_seed=seed, distance_mask=distance_mask, coop_gamma=coop_gamma)
+                                   rng_seed=seed, distance_mask=distance_mask, coop_gamma=coop_gamma, env0=env0,
+                                   n_env_total=n_env_total)
         self.device = self.engine.device
         self._reset_host_buffer(False)
         e = self.engine

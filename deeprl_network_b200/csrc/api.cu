@@ -17,8 +17,10 @@ extern "C" const char* nmarl_last_error(void) { return g_err; }
 // are nmarl_head_width(n_a) floats wide); 105: nmarl_a2c_bptt always computes the heads; the bwd_args field and the
 // entry point that chose whether it did are gone; 106: nmarl_bwd_args.raw_tiles is gone (sv_dzT / sv_dpT always hold
 // one raw tile per 32 rows, half the size), and state_fm must match the layout the path runs; 107: per-env scenario
-// parameters (nmarl_cacc_env_par, nmarl_cacc_draw_par, nmarl_cacc_reset_pe / nmarl_cacc_step_pe)
-extern "C" int nmarl_version(void) { return 107; }
+// parameters (nmarl_cacc_env_par, nmarl_cacc_draw_par, nmarl_cacc_reset_pe / nmarl_cacc_step_pe); 108: envs sharded
+// over processes: nmarl_fwd_args.env0 / B_total key the sampling lanes by the global env index, and
+// nmarl_cacc_reset_shard / nmarl_cacc_reset_pe_shard / nmarl_cacc_draw_par_shard the env draws
+extern "C" int nmarl_version(void) { return 108; }
 extern "C" int nmarl_sizeof_model(void) { return (int)sizeof(nmarl_model); }
 extern "C" int nmarl_sizeof_agent(void) { return (int)sizeof(nmarl_agent); }
 extern "C" int nmarl_sizeof_cacc_cfg(void) { return (int)sizeof(nmarl_cacc_cfg); }

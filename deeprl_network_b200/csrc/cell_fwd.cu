@@ -288,7 +288,7 @@ __global__ void __launch_bounds__(H / 4 * TY) cell_fwd_kernel(const __grid_const
       } else {                                                          // np.random.choice(p=pi): cdf.searchsorted(u,'right')
         double u;
         if (a.sample_mode == NMARL_SAMPLE_UNIFORM) u = a.uniforms[row];
-        else u = philox_u01(a.rng[0], a.rng[1] + a.rng_offset, (uint32_t)row, 0x41435431u);
+        else u = philox_u01(a.rng[0], a.rng[1] + a.rng_offset, nmarl_sample_lane(a, i, b), 0x41435431u);
         double cdf[HW];
         double s = 0.0;
         for (int c = 0; c < n_a; ++c) { s += (double)pi[c]; cdf[c] = s; }
@@ -410,6 +410,17 @@ int dispatch_fwd(const nmarl_model* m, const FwdK& k, cudaStream_t st) {
   return 1;
 }
 
+// The sampling lanes agent * B_total + env0 + env (nmarl_sample_lane) of every agent and env fit the 32-bit counter word.
+int check_sample_lanes(const nmarl_model* m, const nmarl_fwd_args* a) {
+  const int64_t bt = a->B_total > 0 ? a->B_total : a->B;
+  NMARL_CHECK(a->B_total >= 0 && a->env0 >= 0 && (int64_t)a->env0 + a->B <= bt,
+              "policy_step_p: envs env0 %d + B %d must lie inside B_total %d (0 = B)", a->env0, a->B, a->B_total);
+  NMARL_CHECK((int64_t)m->n_agent * bt <= ((int64_t)1 << 32),
+              "policy_step_p: sampling lanes n_agent %d x B_total %lld exceed the 32-bit lane word", m->n_agent,
+              (long long)bt);
+  return 0;
+}
+
 int check_model(const nmarl_model* m) {
   NMARL_CHECK(m != nullptr, "model is NULL");
   NMARL_CHECK(m->n_agent > 0 && m->n_agent <= NMARL_MAX_AGENT, "n_agent %d out of range", m->n_agent);
@@ -455,6 +466,7 @@ extern "C" int nmarl_policy_step_p(const nmarl_model* m, const nmarl_fwd_args* a
   NMARL_CHECK(a->sample_mode != NMARL_SAMPLE_UNIFORM || a->uniforms, "policy_step_p: uniforms required");
   NMARL_CHECK(a->sample_mode != NMARL_SAMPLE_PHILOX || a->rng, "policy_step_p: rng state required");
   NMARL_CHECK(a->state_fm == nmarl_state_fm(m, nmarl_tc_fwd_supported(m, a)), "policy_step_p: " NMARL_STATE_FM_RULE, a->state_fm);
+  if (check_sample_lanes(m, a)) return 1;
   if (a->sv_sh != nullptr) {                 // rollout p-call that also saves activations for BPTT
     NMARL_CHECK(nmarl_tc_fwd_supported(m, a), "policy_step_p: activation saving needs the tensor-core path (B %% 128 == 0, wpack)");
     NMARL_CHECK(a->sv_xin && a->sv_gates, "policy_step_p: sv_xin / sv_gates missing");

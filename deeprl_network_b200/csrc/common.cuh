@@ -201,3 +201,10 @@ __device__ __forceinline__ double philox_u01(uint64_t seed, uint64_t ctr, uint32
   philox4x32_10(c, (uint32_t)seed, (uint32_t)(seed >> 32));
   return u01_from_bits(c[0], c[1]);
 }
+// Philox lane of agent i's action draw in env b of a policy call: the GLOBAL env index keys it (nmarl_fwd_args env0 /
+// B_total), so a process holding envs env0 .. env0 + B - 1 of a sharded run draws what one process holding all does.
+// nmarl_policy_step_p (check_sample_lanes, cell_fwd.cu) has checked that every lane fits 32 bits.
+__device__ __forceinline__ uint32_t nmarl_sample_lane(const nmarl_fwd_args& a, int i, int b) {
+  const uint32_t bt = a.B_total > 0 ? (uint32_t)a.B_total : (uint32_t)a.B;
+  return (uint32_t)i * bt + (uint32_t)a.env0 + (uint32_t)b;
+}

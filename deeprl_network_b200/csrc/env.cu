@@ -62,13 +62,13 @@ __device__ __forceinline__ void write_obs(const nmarl_cacc_cfg& c, const P& p, i
 }
 
 // PE: env b's scenario parameters come from par[b] (nmarl_cacc_reset_pe); without it, from the config.  par is the
-// last parameter so that the other parameters keep their offsets and the PE = false code is that of the config-only
-// kernel.
+// last parameter but one so that the other parameters keep their offsets and the PE = false code is that of the
+// config-only kernel.  env0: global index of env 0 (the Philox lane of env b is env0 + b).
 template <bool PE>
 __global__ void cacc_reset_kernel(const EnvK k, const double* __restrict__ u01, const float* __restrict__ mask,
                                   uint64_t seed, int32_t* episode, double* hs, double* vs, double* us, int32_t* t,
                                   int32_t* collision, double* v_init, float* obs, int obs_stride, float* fp, int n_a,
-                                  const nmarl_cacc_env_par* __restrict__ par) {
+                                  const nmarl_cacc_env_par* __restrict__ par, int env0) {
   const int b = blockIdx.x * blockDim.x + threadIdx.x;
   const int B = k.B;
   if (b >= B) return;
@@ -81,7 +81,7 @@ __global__ void cacc_reset_kernel(const EnvK k, const double* __restrict__ u01, 
   uint32_t ep = 0;
   if (episode != nullptr) { ep = (uint32_t)episode[b]; episode[b] = (int32_t)(ep + 1); }
   for (int p = 0; p < P; ++p) {
-    const double u = (u01 != nullptr) ? u01[(size_t)p * B + b] : philox_u01(seed, ((uint64_t)ep << 8) | (uint64_t)p, (uint32_t)b, 0x454e5601u);
+    const double u = (u01 != nullptr) ? u01[(size_t)p * B + b] : philox_u01(seed, ((uint64_t)ep << 8) | (uint64_t)p, (uint32_t)env0 + (uint32_t)b, 0x454e5601u);
     const double scale = 1.5 + u;
     v_init[(size_t)p * B + b] = (pr.scenario == NMARL_SLOWDOWN) ? pr.v_star * scale : pr.v_star;
     for (int pos = 0; pos < L; ++pos) {
@@ -264,9 +264,10 @@ __global__ void __launch_bounds__(32 * ENV_ROWS) cacc_step_kernel(const EnvK k, 
 }
 
 // One thread per env: the rows of the masked envs for the episode each is about to start (see nmarl_cacc_draw_par).
+// env0: global index of env 0 (the Philox lane of env b is env0 + b).
 __global__ void cacc_draw_par_kernel(const nmarl_cacc_par_ranges r, int scenario, int B, uint64_t seed,
                                      const int32_t* __restrict__ episode, const float* __restrict__ mask,
-                                     nmarl_cacc_env_par* __restrict__ par) {
+                                     nmarl_cacc_env_par* __restrict__ par, int env0) {
   const int b = blockIdx.x * blockDim.x + threadIdx.x;
   if (b >= B) return;
   if (mask != nullptr && mask[b] == 0.0f) return;
@@ -274,11 +275,11 @@ __global__ void cacc_draw_par_kernel(const nmarl_cacc_par_ranges r, int scenario
   double v[NMARL_ENV_PAR_FIELDS];
 #pragma unroll
   for (int k = 0; k < NMARL_ENV_PAR_FIELDS; ++k) {
-    const double u = philox_u01(seed, (ep << 8) | (uint64_t)k, (uint32_t)b, 0x454e5650u);
+    const double u = philox_u01(seed, (ep << 8) | (uint64_t)k, (uint32_t)env0 + (uint32_t)b, 0x454e5650u);
     v[k] = r.lo[k] + u * (r.hi[k] - r.lo[k]);
   }
   if (r.slowdown_prob >= 0.0) {
-    const double u = philox_u01(seed, (ep << 8) | (uint64_t)NMARL_ENV_PAR_FIELDS, (uint32_t)b, 0x454e5650u);
+    const double u = philox_u01(seed, (ep << 8) | (uint64_t)NMARL_ENV_PAR_FIELDS, (uint32_t)env0 + (uint32_t)b, 0x454e5650u);
     scenario = (u < r.slowdown_prob) ? NMARL_SLOWDOWN : NMARL_CATCHUP;
   }
   nmarl_cacc_env_par e;
@@ -293,18 +294,19 @@ __global__ void cacc_draw_par_kernel(const nmarl_cacc_par_ranges r, int scenario
 static int cacc_reset(const nmarl_cacc_cfg* cfg, const nmarl_cacc_env_par* par, int B, const double* u01,
                       const float* mask, uint64_t seed, int32_t* episode, double* hs, double* vs, double* us,
                       int32_t* t, int32_t* collision, double* v_init, float* obs, int obs_stride, float* fp, int n_a,
-                      void* stream) {
+                      void* stream, int env0) {
   NMARL_CHECK(cfg && B > 0, "cacc_reset: bad arguments");
+  NMARL_CHECK(env0 >= 0, "cacc_reset: env0 %d < 0", env0);
   NMARL_CHECK(cfg->platoon_len > 0 && cfg->n_agent % cfg->platoon_len == 0, "cacc_reset: n_agent %% platoon_len != 0");
   NMARL_CHECK(obs_stride >= 5, "cacc_reset: obs_stride < 5");
   EnvK k{*cfg, B};
   const int nt = 64;
   if (par != nullptr)
     cacc_reset_kernel<true><<<(B + nt - 1) / nt, nt, 0, (cudaStream_t)stream>>>(
-        k, u01, mask, seed, episode, hs, vs, us, t, collision, v_init, obs, obs_stride, fp, n_a, par);
+        k, u01, mask, seed, episode, hs, vs, us, t, collision, v_init, obs, obs_stride, fp, n_a, par, env0);
   else
     cacc_reset_kernel<false><<<(B + nt - 1) / nt, nt, 0, (cudaStream_t)stream>>>(
-        k, u01, mask, seed, episode, hs, vs, us, t, collision, v_init, obs, obs_stride, fp, n_a, nullptr);
+        k, u01, mask, seed, episode, hs, vs, us, t, collision, v_init, obs, obs_stride, fp, n_a, nullptr, env0);
   NMARL_LAUNCH_CHECK();
   return 0;
 }
@@ -328,11 +330,19 @@ static int cacc_step(const nmarl_cacc_cfg* cfg, const nmarl_cacc_env_par* par, i
   return 0;
 }
 
+extern "C" int nmarl_cacc_reset_shard(const nmarl_cacc_cfg* cfg, int B, const double* u01, const float* mask,
+                                      uint64_t seed, int32_t* episode, double* hs, double* vs, double* us, int32_t* t,
+                                      int32_t* collision, double* v_init, float* obs, int obs_stride, float* fp, int n_a,
+                                      void* stream, int env0) {
+  return cacc_reset(cfg, nullptr, B, u01, mask, seed, episode, hs, vs, us, t, collision, v_init, obs, obs_stride, fp,
+                    n_a, stream, env0);
+}
+
 extern "C" int nmarl_cacc_reset(const nmarl_cacc_cfg* cfg, int B, const double* u01, const float* mask, uint64_t seed,
                                 int32_t* episode, double* hs, double* vs, double* us, int32_t* t, int32_t* collision,
                                 double* v_init, float* obs, int obs_stride, float* fp, int n_a, void* stream) {
-  return cacc_reset(cfg, nullptr, B, u01, mask, seed, episode, hs, vs, us, t, collision, v_init, obs, obs_stride, fp,
-                    n_a, stream);
+  return nmarl_cacc_reset_shard(cfg, B, u01, mask, seed, episode, hs, vs, us, t, collision, v_init, obs, obs_stride,
+                                fp, n_a, stream, 0);
 }
 
 extern "C" int nmarl_cacc_step(const nmarl_cacc_cfg* cfg, int B, int train_mode, const int32_t* action, double* hs,
@@ -342,13 +352,22 @@ extern "C" int nmarl_cacc_step(const nmarl_cacc_cfg* cfg, int B, int train_mode,
                    greward, done, stream);
 }
 
+extern "C" int nmarl_cacc_reset_pe_shard(const nmarl_cacc_cfg* cfg, const nmarl_cacc_env_par* par, int B,
+                                         const double* u01, const float* mask, uint64_t seed, int32_t* episode,
+                                         double* hs, double* vs, double* us, int32_t* t, int32_t* collision,
+                                         double* v_init, float* obs, int obs_stride, float* fp, int n_a, void* stream,
+                                         int env0) {
+  NMARL_CHECK(par != nullptr, "cacc_reset_pe: par is NULL");
+  return cacc_reset(cfg, par, B, u01, mask, seed, episode, hs, vs, us, t, collision, v_init, obs, obs_stride, fp,
+                    n_a, stream, env0);
+}
+
 extern "C" int nmarl_cacc_reset_pe(const nmarl_cacc_cfg* cfg, const nmarl_cacc_env_par* par, int B, const double* u01,
                                    const float* mask, uint64_t seed, int32_t* episode, double* hs, double* vs,
                                    double* us, int32_t* t, int32_t* collision, double* v_init, float* obs,
                                    int obs_stride, float* fp, int n_a, void* stream) {
-  NMARL_CHECK(par != nullptr, "cacc_reset_pe: par is NULL");
-  return cacc_reset(cfg, par, B, u01, mask, seed, episode, hs, vs, us, t, collision, v_init, obs, obs_stride, fp,
-                    n_a, stream);
+  return nmarl_cacc_reset_pe_shard(cfg, par, B, u01, mask, seed, episode, hs, vs, us, t, collision, v_init, obs,
+                                   obs_stride, fp, n_a, stream, 0);
 }
 
 extern "C" int nmarl_cacc_step_pe(const nmarl_cacc_cfg* cfg, const nmarl_cacc_env_par* par, int B, int train_mode,
@@ -360,11 +379,12 @@ extern "C" int nmarl_cacc_step_pe(const nmarl_cacc_cfg* cfg, const nmarl_cacc_en
                    greward, done, stream);
 }
 
-extern "C" int nmarl_cacc_draw_par(const nmarl_cacc_cfg* cfg, const nmarl_cacc_par_ranges* ranges, int B,
-                                   uint64_t seed, const int32_t* episode, const float* mask, nmarl_cacc_env_par* par,
-                                   void* stream) {
+extern "C" int nmarl_cacc_draw_par_shard(const nmarl_cacc_cfg* cfg, const nmarl_cacc_par_ranges* ranges, int B,
+                                         uint64_t seed, const int32_t* episode, const float* mask,
+                                         nmarl_cacc_env_par* par, void* stream, int env0) {
   static const char* const name[NMARL_ENV_PAR_FIELDS] = {"h_star", "v_star", "h_s", "h_g", "v_max", "u_min", "u_max"};
   NMARL_CHECK(cfg && ranges && par && B > 0, "cacc_draw_par: bad arguments");
+  NMARL_CHECK(env0 >= 0, "cacc_draw_par: env0 %d < 0", env0);
   const nmarl_cacc_par_ranges& r = *ranges;
   for (int k = 0; k < NMARL_ENV_PAR_FIELDS; ++k)
     NMARL_CHECK(r.lo[k] <= r.hi[k], "cacc_draw_par: %s range [%g, %g] needs lo <= hi", name[k], r.lo[k], r.hi[k]);
@@ -378,7 +398,13 @@ extern "C" int nmarl_cacc_draw_par(const nmarl_cacc_cfg* cfg, const nmarl_cacc_p
   NMARL_CHECK(r.slowdown_prob <= 1.0, "cacc_draw_par: slowdown_prob %g > 1", r.slowdown_prob);
   const int nt = 128;
   cacc_draw_par_kernel<<<(B + nt - 1) / nt, nt, 0, (cudaStream_t)stream>>>(r, cfg->scenario, B, seed, episode, mask,
-                                                                          par);
+                                                                          par, env0);
   NMARL_LAUNCH_CHECK();
   return 0;
+}
+
+extern "C" int nmarl_cacc_draw_par(const nmarl_cacc_cfg* cfg, const nmarl_cacc_par_ranges* ranges, int B,
+                                   uint64_t seed, const int32_t* episode, const float* mask, nmarl_cacc_env_par* par,
+                                   void* stream) {
+  return nmarl_cacc_draw_par_shard(cfg, ranges, B, seed, episode, mask, par, stream, 0);
 }

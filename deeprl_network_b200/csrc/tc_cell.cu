@@ -387,7 +387,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_cell_fwd_kernel(const __grid
         } else {
           double u;
           if (a.sample_mode == NMARL_SAMPLE_UNIFORM) u = a.uniforms[row];
-          else u = philox_u01(a.rng[0], a.rng[1] + a.rng_offset, (uint32_t)row, 0x41435431u);
+          else u = philox_u01(a.rng[0], a.rng[1] + a.rng_offset, nmarl_sample_lane(a, i, b), 0x41435431u);
           double cdf[HW];
           double s = 0.0;
 #pragma unroll

@@ -8,7 +8,7 @@ lives in device memory as float64 [agent][env] arrays and is advanced by the ``n
 kernels (csrc/env.cu); ``*_device`` methods expose the batched tensors without host copies.
 
 New optional keys in ``ENV_CONFIG`` (everything else parses exactly like the reference):
-  n_env        parallel episodes on this process (default 1)
+  n_env        parallel episodes in total (default 1); a process of a sharded run holds n_env / world of them
   platoon_len  vehicles per platoon (default n_vehicle); < n_vehicle gives several independent
                platoons -- used only by the synthetic 5x5-grid configuration
   topology     'chain' (default) or 'grid' (row-major 4-neighbour grid, Manhattan distance)
@@ -112,12 +112,20 @@ def parse_env_par(config, h_min=None):
 
 
 class CACCEnv:
-    def __init__(self, config, n_env=None, device=None):
+    def __init__(self, config, n_env=None, device=None, env0=0, n_env_total=None):
+        """n_env overrides ENV_CONFIG.n_env.  A shard of a run over several processes holds the n_env envs
+        env0 .. env0 + n_env - 1 of n_env_total: its random draws (initial conditions, per-env parameters) are keyed
+        by the global env index, so they are those of the same envs in one process holding all n_env_total."""
         L.require_cuda()
         self._load_config(config)
         if n_env is not None:
             self.n_env = int(n_env)
-        if self.par_spec is not None and self.n_env == 1:
+        self.env0 = int(env0)
+        self.n_env_total = self.n_env if n_env_total is None else int(n_env_total)
+        if not (self.env0 >= 0 and self.env0 + self.n_env <= self.n_env_total):
+            raise ValueError('envs %d .. %d are not inside the %d envs of the run'
+                             % (self.env0, self.env0 + self.n_env - 1, self.n_env_total))
+        if self.par_spec is not None and self.n_env_total == 1:
             raise ValueError('ENV_CONFIG keys %s (per-env scenario parameters) need batched training: set n_env > 1 '
                              '(VecTrainer); the one-env Trainer runs the nominal values only'
                              % ', '.join(env_par_keys(config)))
@@ -231,19 +239,21 @@ class CACCEnv:
         seed = int(self.cfg_seed if philox_seed is None else philox_seed) & (2 ** 64 - 1)
         if self.env_par is not None:
             # the reset envs draw their parameters for the episode they start (Philox keyed by seed, env, episode)
-            L.check(L.lib().nmarl_cacc_draw_par(C.byref(self.cfg), C.byref(self._par_ranges), self.n_env, seed,
-                                                L.ptr(self.episode_dev), L.ptr(mask), L.ptr(self.env_par),
-                                                L.stream()), 'nmarl_cacc_draw_par')
-            L.check(L.lib().nmarl_cacc_reset_pe(C.byref(self.cfg), L.ptr(self.env_par), self.n_env, L.ptr(u01),
-                                                L.ptr(mask), seed, L.ptr(self.episode_dev), L.ptr(self.hs),
-                                                L.ptr(self.vs), L.ptr(self.us), L.ptr(self.t_dev),
-                                                L.ptr(self.collision_dev), L.ptr(self.v_init), L.ptr(obs),
-                                                obs.shape[-1], L.ptr(fp), self.n_a, L.stream()), 'nmarl_cacc_reset_pe')
+            L.check(L.lib().nmarl_cacc_draw_par_shard(C.byref(self.cfg), C.byref(self._par_ranges), self.n_env, seed,
+                                                      L.ptr(self.episode_dev), L.ptr(mask), L.ptr(self.env_par),
+                                                      L.stream(), self.env0), 'nmarl_cacc_draw_par_shard')
+            L.check(L.lib().nmarl_cacc_reset_pe_shard(C.byref(self.cfg), L.ptr(self.env_par), self.n_env, L.ptr(u01),
+                                                      L.ptr(mask), seed, L.ptr(self.episode_dev), L.ptr(self.hs),
+                                                      L.ptr(self.vs), L.ptr(self.us), L.ptr(self.t_dev),
+                                                      L.ptr(self.collision_dev), L.ptr(self.v_init), L.ptr(obs),
+                                                      obs.shape[-1], L.ptr(fp), self.n_a, L.stream(), self.env0),
+                    'nmarl_cacc_reset_pe_shard')
             return
-        L.check(L.lib().nmarl_cacc_reset(C.byref(self.cfg), self.n_env, L.ptr(u01), L.ptr(mask), seed,
-                                         L.ptr(self.episode_dev), L.ptr(self.hs), L.ptr(self.vs), L.ptr(self.us),
-                                         L.ptr(self.t_dev), L.ptr(self.collision_dev), L.ptr(self.v_init),
-                                         L.ptr(obs), obs.shape[-1], L.ptr(fp), self.n_a, L.stream()), 'nmarl_cacc_reset')
+        L.check(L.lib().nmarl_cacc_reset_shard(C.byref(self.cfg), self.n_env, L.ptr(u01), L.ptr(mask), seed,
+                                               L.ptr(self.episode_dev), L.ptr(self.hs), L.ptr(self.vs), L.ptr(self.us),
+                                               L.ptr(self.t_dev), L.ptr(self.collision_dev), L.ptr(self.v_init),
+                                               L.ptr(obs), obs.shape[-1], L.ptr(fp), self.n_a, L.stream(), self.env0),
+                'nmarl_cacc_reset_shard')
 
     def step_device(self, action, obs_out=None, reward_out=None, greward_out=None, done_out=None):
         """action int32 [N,B] device tensor.  Outputs default to the env's own buffers."""
@@ -274,10 +284,11 @@ class CACCEnv:
         out['scenario'] = t.view(torch.int32)[:, 2 * len(L.ENV_PAR_FIELDS)].numpy()
         return out
 
-    def par_stats(self):
+    def par_stats(self, tab=None):
         """Mean, min and max over the batch of every drawn field (and of `slowdown`: 1 for a slow-down env), as one
-        flat record {<field>_mean, <field>_min, <field>_max}.  Host sync."""
-        tab = self.par_table()
+        flat record {<field>_mean, <field>_min, <field>_max}.  tab: a table in the layout of par_table() (the rows of
+        every shard of a sharded run); default this env's own.  Host sync."""
+        tab = dict(self.par_table() if tab is None else tab)
         tab['slowdown'] = (tab.pop('scenario') == L.SLOWDOWN).astype(np.float64)
         rec = {}
         for f, v in tab.items():

@@ -21,6 +21,7 @@ import numpy as np
 import torch
 
 from . import _lib as L
+from . import dist as D
 from .agents.engine import PolicyEngine
 from .envs.cacc_env import CACCEnv, control_record, env_par_keys, nominal_config, traffic_frame, write_records
 from .layout import ModelLayout
@@ -281,6 +282,10 @@ class VecTrainer:
     training forward/BPTT/wgrad -> [all-reduce] -> clip + RMSProp, then per-env auto-reset of the
     environments whose episode ended (model.reset() + env.reset() of the reference, per env).
     With ``graph=True`` one update is captured once into a CUDA graph and replayed.
+
+    When the env is one shard of a run over several processes (env.n_env_total > env.n_env), the records gather
+    every rank's envs to rank 0 in global env order and are computed there on what one process would hold; the other
+    ranks record nothing.
     """
 
     def __init__(self, env, model, graph=True, sample='philox'):
@@ -347,12 +352,21 @@ class VecTrainer:
     def log_rewards(self, global_step, summary_writer=None):
         """One `train_reward.csv` record (same columns as Trainer._log_episode): mean / std of the per-step global
         reward over the last batch of every env.  Unlike the one-env Trainer (quirk Q4) no greedy test episode is
-        interleaved: these are the TRAINING rewards.  Host sync."""
+        interleaved: these are the TRAINING rewards.  Host sync.  Returns the mean (None on ranks other than 0 of a
+        sharded run)."""
         g = self.engine.grew_buf[:self.engine.T_cur]
+        tab = self.env.par_table() if getattr(self.env, 'env_par', None) is not None else None
+        if self.env.n_env_total != self.env.n_env:
+            parts = D.gather_to_root((g.cpu().numpy(), tab))
+            if parts is None:
+                return None
+            g = torch.from_numpy(np.concatenate([p[0] for p in parts], axis=1)).to(g.device)
+            if tab is not None:
+                tab = {k: np.concatenate([p[1][k] for p in parts]) for k in tab}
         mean, std = float(g.mean().item()), float(g.std(unbiased=False).item())
         self.data.append(dict(agent=self.env.agent, step=int(global_step), test_id=-1, avg_reward=mean, std_reward=std))
-        if getattr(self.env, 'env_par', None) is not None:
-            self.par_data.append(dict(step=int(global_step), **self.env.par_stats()))
+        if tab is not None:
+            self.par_data.append(dict(step=int(global_step), **self.env.par_stats(tab)))
         if summary_writer is not None:
             summary_writer.add_scalar('train_reward', mean, int(global_step))
         return mean
@@ -385,9 +399,13 @@ class BatchedEvaluator:
 
     Evaluation always runs the config's nominal scenario parameters: per-env parameter keys (``*_range``,
     ``slowdown_prob``) of a training config are ignored here, so test rewards stay comparable across runs.
+
+    In a run over several processes (``world`` > 1) ``test_rewards`` runs rank ``rank``'s contiguous part of the
+    seeds and reduces every rank's episodes on rank 0, in seed order.
     """
 
-    def __init__(self, env_config, model, output_path=None, max_env=4096, record_bytes=2 ** 31, graph=True):
+    def __init__(self, env_config, model, output_path=None, max_env=4096, record_bytes=2 ** 31, graph=True, world=1,
+                 rank=0):
         if env_par_keys(env_config):
             env_config = nominal_config(env_config)
         self.config, self.model, self.output_path = env_config, model, output_path
@@ -396,6 +414,7 @@ class BatchedEvaluator:
         self.agent = env_config.get('agent')
         self._runners = {}
         self.data = []                     # test_reward.csv records (log_test)
+        self.world, self.rank = int(world), int(rank)
 
     @staticmethod
     def _eval_layout(lay):
@@ -494,13 +513,24 @@ class BatchedEvaluator:
                               self.config.getfloat('control_interval_sec'))
 
     def test_rewards(self, seeds):
-        """mean / std of the per-step global rewards of one greedy episode per seed, all episodes together."""
-        r = np.concatenate([reward[1:] for _, _, _, reward, _ in self.episodes(list(seeds))])
+        """mean / std of the per-step global rewards of one greedy episode per seed, all episodes together (None on
+        ranks other than 0 of a run over several processes)."""
+        mine = [reward[1:] for _, _, _, reward, _ in self.episodes(D.seed_shard(seeds, self.world, self.rank))]
+        if self.world > 1:
+            parts = D.gather_to_root(mine)
+            if parts is None:
+                return None
+            mine = [r for part in parts for r in part]
+        r = np.concatenate(mine)
         return np.mean(r), np.std(r)
 
     def log_test(self, global_step, seeds, summary_writer=None):
-        """One test_reward.csv record (columns of train_reward.csv) and the TB scalar `test_reward`."""
-        mean, std = self.test_rewards(seeds)
+        """One test_reward.csv record (columns of train_reward.csv) and the TB scalar `test_reward`.  Returns the
+        mean (None on ranks other than 0 of a run over several processes)."""
+        out = self.test_rewards(seeds)
+        if out is None:
+            return None
+        mean, std = out
         self.data.append(dict(agent=self.agent, step=int(global_step), test_id=-1, avg_reward=mean, std_reward=std))
         if summary_writer is not None:
             summary_writer.add_scalar('test_reward', mean, int(global_step))

@@ -172,6 +172,19 @@ int nmarl_cacc_step_pe(const nmarl_cacc_cfg* cfg, const nmarl_cacc_env_par* par,
  * every draw (h_min < lo[h_s], hi[h_s] < lo[h_g]); u_min < 0 < u_max; v_star > 0; h_star > 0; slowdown_prob <= 1. */
 int nmarl_cacc_draw_par(const nmarl_cacc_cfg* cfg, const nmarl_cacc_par_ranges* ranges, int B, uint64_t seed,
                         const int32_t* episode, const float* mask, nmarl_cacc_env_par* par, void* stream);
+/* Envs sharded over processes: the same three calls for the global envs env0 .. env0 + B - 1 (the Philox lane of env
+ * b is env0 + b, so a shard draws exactly what those envs of one process holding all of them draw).  The unsuffixed
+ * calls are these with env0 = 0.  Refused unless env0 >= 0 (env0 + B - 1 then always fits the 32-bit lane word).   */
+int nmarl_cacc_reset_shard(const nmarl_cacc_cfg* cfg, int B, const double* u01, const float* mask, uint64_t seed,
+                           int32_t* episode, double* hs, double* vs, double* us, int32_t* t, int32_t* collision,
+                           double* v_init, float* obs, int obs_stride, float* fp, int n_a, void* stream, int env0);
+int nmarl_cacc_reset_pe_shard(const nmarl_cacc_cfg* cfg, const nmarl_cacc_env_par* par, int B, const double* u01,
+                              const float* mask, uint64_t seed, int32_t* episode, double* hs, double* vs, double* us,
+                              int32_t* t, int32_t* collision, double* v_init, float* obs, int obs_stride, float* fp,
+                              int n_a, void* stream, int env0);
+int nmarl_cacc_draw_par_shard(const nmarl_cacc_cfg* cfg, const nmarl_cacc_par_ranges* ranges, int B, uint64_t seed,
+                              const int32_t* episode, const float* mask, nmarl_cacc_env_par* par, void* stream,
+                              int env0);
 
 /* ---- K2-K6: fused message-gather + encoders + LSTM cell + heads ----------------------------
  * Replaces lstm / lstm_comm / lstm_ic3 / lstm_dial (agents/utils.py:87-115,118-217,344-417,
@@ -198,13 +211,15 @@ typedef struct {
                            /* Keying, which any other binding has to match: Philox4x32-10 with  */
                            /* key = (seed low, seed high) and counter words = (c low, c high,   */
                            /* lane, 0x41435431), c = rng[1] + rng_offset (mod 2^64), lane =     */
-                           /* agent * B + env; u = ((w0 >> 5) * 2^26 + (w1 >> 6)) / 2^53 from   */
-                           /* output words 0, 1.  The call does not move rng[1]: a rollout      */
-                           /* passes offsets 0..T and then calls nmarl_rng_advance(rng, T + 1). */
+                           /* agent * B_total + env0 + env (the GLOBAL env index; env0 = 0 and  */
+                           /* B_total = B unless the envs are sharded over processes);          */
+                           /* u = ((w0 >> 5) * 2^26 + (w1 >> 6)) / 2^53 from output words 0, 1. */
+                           /* The call does not move rng[1]: a rollout passes offsets 0..T and  */
+                           /* then calls nmarl_rng_advance(rng, T + 1).                          */
                            /* nmarl_cacc_reset draws from the same generator with counter =     */
-                           /* episode << 8 | platoon, lane = env and the tag 0x454e5601, and    */
-                           /* nmarl_cacc_draw_par with counter = episode << 8 | parameter k,     */
-                           /* lane = env and the tag 0x454e5650                                  */
+                           /* episode << 8 | platoon, lane = env0 + env and the tag 0x454e5601, */
+                           /* and nmarl_cacc_draw_par with counter = episode << 8 | parameter k, */
+                           /* lane = env0 + env and the tag 0x454e5650 (env0: the *_shard calls) */
   const int32_t* act_in;   /* v-call: [N][B] same-step actions                                 */
   float* v;                /* v-call: [N][B]                                                   */
   const float* wpack;      /* packed 3xTF32 operands (nmarl_pack_weights) or NULL.  When set and  */
@@ -216,6 +231,12 @@ typedef struct {
   float* sv_xin; float* sv_sh; float* sv_gates; float* sv_enc;   /* step-t slices, see nmarl_bwd_args      */
   int32_t state_fm;        /* layout of c/h: 1 = feature-major [N][64][B], required on the tensor-  */
                            /* core path except for DIAL; 0 = env-major, required everywhere else */
+  /* envs sharded over processes: this call's B envs are the global envs env0 .. env0 + B - 1 of B_total, and the
+   * sampling lane is keyed by the global index (see rng above), so that a sharded run samples what one process
+   * holding all B_total envs samples.  B_total = 0 means B.  Refused unless env0 >= 0, env0 + B <= B_total and
+   * every lane fits the 32-bit counter word (n_agent * B_total <= 2^32).                                        */
+  int32_t env0;
+  int32_t B_total;
 } nmarl_fwd_args;
 
 int nmarl_policy_step_p(const nmarl_model* m, const nmarl_fwd_args* a, void* stream);

@@ -6,13 +6,20 @@ The reference's command line is kept verbatim (main.py:21-40 there) so existing 
     python main.py --base-dir D evaluate [--evaluation-seeds s1,s2,...] [--demo]
 
 and so is the .ini surface (MODEL_CONFIG / TRAIN_CONFIG / ENV_CONFIG).  Optional new keys: ENV_CONFIG.n_env
-(parallel episodes per process) and TRAIN_CONFIG.greedy_test (default false).  n_env = 1 runs the reference's
+(parallel episodes in total) and TRAIN_CONFIG.greedy_test (default false).  n_env = 1 runs the reference's
 one-episode-at-a-time Trainer; n_env > 1 the device-resident VecTrainer, which with greedy_test also logs the greedy
 test reward over ENV_CONFIG.test_seeds to data/test_reward.csv.  With n_env > 1, ENV_CONFIG.<key>_range / slowdown_prob
 give every env its own scenario parameters, redrawn at each of its resets (data/env_par.csv records what was drawn);
 evaluation keeps the nominal values.  evaluate runs all seeds at once on the device and
 writes the files the reference's one-seed-at-a-time Evaluator writes.  Agents: ia2c, ia2c_fp, ma2c_cu, ma2c_nc, ma2c_ic3, ma2c_dial on the CACC scenarios;
 ATSC/SUMO environments are out of scope (SURVEY row 10).
+
+train also runs on all the GPUs of a node under torchrun, e.g. `torchrun --standalone --nproc-per-node 8 main.py
+--base-dir D train --config-dir F.ini`: rank r of W trains the envs [r n_env / W, (r + 1) n_env / W) of ENV_CONFIG.n_env
+and the gradient is summed over the ranks, which gives the training run of one process with the same .ini up to the
+order of floating-point sums.  Rank 0 alone writes the log, the files under data/ and the checkpoint.  NCCL when every
+rank has a GPU of its own, else gloo (ranks sharing a GPU; no CUDA graphs).  Refused with a ValueError: n_env not
+divisible by the process count, n_env = 1, and evaluate under torchrun (INTEGRATION §4).
 """
 import argparse
 import configparser
@@ -21,6 +28,7 @@ import os
 
 from deeprl_network_b200.agents import models as agent_models
 from deeprl_network_b200.envs.cacc_env import CACCEnv, nominal_config
+from deeprl_network_b200 import dist as D
 from deeprl_network_b200 import utils as U
 
 AGENTS = {'ia2c': agent_models.IA2C, 'ia2c_fp': agent_models.IA2C_FP, 'ma2c_cu': agent_models.IA2C_CU,
@@ -51,11 +59,14 @@ def read_config(path):
     return cfg
 
 
-def init_env(config, port=0):
-    """ENV_CONFIG section -> environment (only the CACC family exists here)."""
+def init_env(config, port=0, shard=None):
+    """ENV_CONFIG section -> environment (only the CACC family exists here).  shard: (env0, n_env) of this process
+    in a run over several processes (ENV_CONFIG.n_env is then the run's total)."""
     if config.get('scenario').startswith('atsc'):
         raise NotImplementedError('ATSC/SUMO environments are outside the accelerated hot path')
-    return CACCEnv(config)
+    if shard is None:
+        return CACCEnv(config)
+    return CACCEnv(config, n_env=shard[1], env0=shard[0], n_env_total=config.getint('n_env'))
 
 
 def init_agent(env, config, total_step, seed, **kw):
@@ -63,60 +74,89 @@ def init_agent(env, config, total_step, seed, **kw):
     if env.agent not in AGENTS:
         logging.error('agent %r is not on the accelerated hot path' % env.agent)
         return None
-    if env.agent == 'ia2c' and env.n_env > 1:     # device-resident rollouts gather neighbour observations in the kernel
+    # device-resident rollouts (n_env > 1 in the run, kw n_env_total for one shard of it) gather neighbour
+    # observations in the kernel
+    if env.agent == 'ia2c' and kw.get('n_env_total', env.n_env) > 1:
         kw.setdefault('obs_mode', 'gather')
     return AGENTS[env.agent](env.n_s_ls, env.n_a_ls, env.neighbor_mask, env.distance_mask, env.coop_gamma,
                              total_step, config, seed=seed, n_env=env.n_env, **kw)
 
 
-def _train_batched(env, model, total_step, log_interval, writer=None, output_path=None, tester=None):
-    """n_env > 1: whole updates on the device until total_step environment steps (summed over envs) are done.
+def _train_batched(env, model, total_step, log_interval, writer=None, output_path=None, tester=None, graph=True):
+    """n_env > 1: whole updates on the device until total_step environment steps (summed over all envs of all
+    processes) are done.
     Every `log_interval` environment steps one record goes to data/train_reward.csv (and the TB scalar
     `train_reward`): mean / std of the per-step global TRAINING reward of the last batch.  With a `tester`
     (BatchedEvaluator, TRAIN_CONFIG.greedy_test) each record also runs one greedy episode per ENV_CONFIG test seed
-    with the current weights and adds a record to data/test_reward.csv (and the TB scalar `test_reward`)."""
-    loop = U.VecTrainer(env, model)
+    with the current weights and adds a record to data/test_reward.csv (and the TB scalar `test_reward`).  In a run over
+    several processes every rank calls it; the records are taken on rank 0 (the others pass output_path None)."""
+    loop = U.VecTrainer(env, model, graph=graph)
     loop.start()
-    done_steps, per_update = 0, model.n_step * env.n_env
+    done_steps, per_update = 0, model.n_step * env.n_env_total
     every = max(1, int(log_interval) // per_update)
     while done_steps < total_step:
         loop.update()
         done_steps += per_update
         if loop.n_update % every == 0 or done_steps >= total_step:
             r = loop.log_rewards(done_steps, writer)
-            logging.info('update %d, env steps %d, mean step reward %.2f' % (loop.n_update, done_steps, r))
+            if r is not None:
+                logging.info('update %d, env steps %d, mean step reward %.2f' % (loop.n_update, done_steps, r))
             if tester is not None:
                 r = tester.log_test(done_steps, env.test_seeds, writer)
-                logging.info('update %d, env steps %d, greedy test reward %.2f' % (loop.n_update, done_steps, r))
+                if r is not None:
+                    logging.info('update %d, env steps %d, greedy test reward %.2f' % (loop.n_update, done_steps, r))
     if output_path is not None:
         loop.write_csv(output_path)
         if tester is not None:
             tester.write_csv(output_path)
+    loop.graph = None          # a captured graph may hold NCCL kernels: release it before the process group goes
     return done_steps
 
 
 def train(args):
-    dirs = U.init_dir(args.base_dir)
-    U.init_log(dirs['log'])
-    U.copy_file(args.config_dir, dirs['data'])             # evaluate finds the config next to the results
+    world, rank, _ = D.launch_world()
+    shard = backend = None
+    if world > 1:
+        # refused on every rank before the process group exists
+        shard = D.env_shard(read_config(args.config_dir).getint('ENV_CONFIG', 'n_env', fallback=1), world, rank)
+        backend = D.init_from_env()
+    lead = rank == 0                                       # rank 0 alone writes the log, data/ and the checkpoint
+    if lead:
+        dirs = U.init_dir(args.base_dir)
+        U.init_log(dirs['log'])
+        U.copy_file(args.config_dir, dirs['data'])         # evaluate finds the config next to the results
+    else:
+        logging.basicConfig(format='%(asctime)s [rank ' + str(rank) + '] %(message)s', level=logging.WARNING)
     cfg = read_config(args.config_dir)
     steps = {k: int(cfg.getfloat('TRAIN_CONFIG', k)) for k in ('total_step', 'test_interval', 'log_interval')}
-    env = init_env(cfg['ENV_CONFIG'])
+    env = init_env(cfg['ENV_CONFIG'], shard=shard)
     logging.info('Training: a dim %r, agent dim: %d' % (env.n_a_ls, env.n_agent))
-    model = init_agent(env, cfg['MODEL_CONFIG'], steps['total_step'], cfg.getint('ENV_CONFIG', 'seed'))
+    shard_kw = {} if shard is None else dict(env0=env.env0, n_env_total=env.n_env_total)
+    model = init_agent(env, cfg['MODEL_CONFIG'], steps['total_step'], cfg.getint('ENV_CONFIG', 'seed'), **shard_kw)
     if model is None:
         raise SystemExit(2)
-    if env.n_env > 1:
+    if world > 1:
+        # every rank built its weights from the config seed; a change of the init order must not split them silently
+        D.check_replicas({'params': model.engine.params})
+        logging.info('Training: %d processes (%s), %d of the %d envs each, tensor-core kernels: %s' % (
+            world, backend, env.n_env, env.n_env_total, model.engine.use_tc))
+    if shard is not None or env.n_env > 1:
         greedy_test = cfg.getboolean('TRAIN_CONFIG', 'greedy_test', fallback=False)
-        tester = U.BatchedEvaluator(cfg['ENV_CONFIG'], model) if greedy_test else None
+        tester = U.BatchedEvaluator(cfg['ENV_CONFIG'], model, world=world, rank=rank) if greedy_test else None
         final_step = _train_batched(env, model, steps['total_step'], steps['log_interval'],
-                                    U.make_summary_writer(dirs['log']), dirs['data'], tester)
+                                    U.make_summary_writer(dirs['log']) if lead else None,
+                                    dirs['data'] if lead else None, tester, graph=backend != 'gloo')
     else:
         counter = U.Counter(steps['total_step'], steps['test_interval'], steps['log_interval'])
         U.Trainer(env, model, counter, U.make_summary_writer(dirs['log']), output_path=dirs['data']).run()
         final_step = counter.cur_step
-    logging.info('Training: save final model at step %d ...' % final_step)
-    model.save(dirs['model'], final_step)
+    if world > 1:
+        D.check_replicas({'params': model.engine.params, 'rmsprop ms': model.engine.ms})
+        logging.info('Training: parameters and RMSProp state are bit-identical on all %d ranks' % world)
+    if lead:
+        logging.info('Training: save final model at step %d ...' % final_step)
+        model.save(dirs['model'], final_step)
+    D.shutdown()
 
 
 def evaluate_fn(agent_dir, output_dir, seeds, port, demo):
@@ -143,6 +183,8 @@ def evaluate_fn(agent_dir, output_dir, seeds, port, demo):
 
 
 def evaluate(args):
+    if D.launch_world()[0] > 1:
+        raise ValueError('main.py evaluate runs in one process (all seeds in one batched pass); start it without torchrun')
     output_dir = None
     if not args.demo:
         dirs = U.init_dir(args.base_dir, pathes=['eva_data', 'eva_log'])
