@@ -17,6 +17,14 @@ import numpy as np
 import torch
 
 from .. import _lib as L
+from .. import dist as D
+
+
+def _same_shape(src, dst, name):
+    if tuple(src.shape) != tuple(dst.shape):
+        raise ValueError('snapshot tensor %s has shape %s, this run needs %s' % (name, tuple(src.shape), tuple(dst.shape)))
+    return src
+
 
 def tc_eligible(layout, n_env):
     """True when a model of this layout with n_env envs runs the tensor-core kernels.  Same conditions as
@@ -189,6 +197,41 @@ class PolicyEngine:
         if bw:
             self.c_bw.copy_(c); self.h_bw.copy_(h)
         self._refresh_msg()
+
+    # ---- snapshots (VecTrainer.snapshot / restore) ------------------------------------------------
+    def snapshot(self):
+        """Host copy of what the next update reads, taken between updates (state slot 0): 'params', 'ms', 'rng' (the
+        same on every rank of a run) and 'envs', this engine's per-env tensors in the canonical env-major layout
+        [agent][env][feature] whatever the kernel path ('env_axis' gives each one's env axis): the recurrent state
+        c / h and c_bw / h_bw, DIAL's message, and slot 0 of the observation, fingerprint and done buffers."""
+        assert self.cur == 0, 'snapshots are taken between updates'
+        em = (lambda t: t.permute(0, 2, 1)) if self.state_fm else (lambda t: t)
+        envs = dict(c=em(self.c[0]), h=em(self.h[0]), c_bw=em(self.c_bw), h_bw=em(self.h_bw), obs=self.obs_buf[0],
+                    fp=self.fp_buf[0], done=self.done_buf[0])
+        if self.msg[0] is not None:
+            envs['msg'] = self.msg[0]
+        return dict(params=self.params.cpu(), ms=self.ms.cpu(), rng=self.rng.cpu(),
+                    envs={k: v.contiguous().cpu() for k, v in envs.items()},
+                    env_axis={k: 0 if k == 'done' else 1 for k in envs})
+
+    def restore(self, snap):
+        """Copy a snapshot into this engine's tensors in place.  Its per-env tensors hold the envs of the whole run in
+        global env order (VecTrainer gathers them); this engine takes its envs env0 .. env0 + B - 1."""
+        if snap['params'].shape != self.params.shape:
+            raise ValueError('the snapshot holds %d parameters, the model %d' % (snap['params'].numel(), self.params.numel()))
+        if ('msg' in snap['envs']) != (self.msg[0] is not None):
+            raise ValueError('the snapshot was taken from another agent')
+        envs = D.take_envs(snap['envs'], snap['env_axis'], self.env0, self.B)
+        em = (lambda t: t.permute(0, 2, 1)) if self.state_fm else (lambda t: t)
+        self.cur = 0
+        for dst, k in ((self.c[0], 'c'), (self.h[0], 'h'), (self.c_bw, 'c_bw'), (self.h_bw, 'h_bw')):
+            dst.copy_(em(_same_shape(envs[k], em(dst), k)))
+        if self.msg[0] is not None:
+            self.msg[0].copy_(_same_shape(envs['msg'], self.msg[0], 'msg'))
+        for dst, k in ((self.obs_buf[0], 'obs'), (self.fp_buf[0], 'fp'), (self.done_buf[0], 'done')):
+            dst.copy_(_same_shape(envs[k], dst, k))
+        self.params.copy_(snap['params']); self.ms.copy_(snap['ms']); self.rng.copy_(snap['rng'])
+        self.repack()
 
     # ---- forward calls ----------------------------------------------------------------------------
     def _fwd_args(self, obs, fp, done):

@@ -20,6 +20,7 @@ import torch
 
 from .. import _lib as L
 from ..layout import HeteroLayout, ModelLayout
+from ..resume import atomic_save
 from .engine import PolicyEngine
 from .utils import Scheduler
 
@@ -207,10 +208,11 @@ class IA2C:
 
     # ---- checkpoints (agents/models.py:53-82; own on-disk format, same naming rule) ---------------------
     def save(self, model_dir, global_step):
+        """<model_dir>/checkpoint-<step>.pt, written under a temporary name and renamed (resume.atomic_save)."""
         e = self.engine
-        torch.save({'variant': self.variant, 'names': [n for n, _, _ in self.layout.entries],
-                    'params': e.params.cpu(), 'ms': e.ms.cpu(), 'global_step': int(global_step)},
-                   model_dir + 'checkpoint-%d.pt' % int(global_step))
+        atomic_save({'variant': self.variant, 'names': [n for n, _, _ in self.layout.entries],
+                     'params': e.params.cpu(), 'ms': e.ms.cpu(), 'global_step': int(global_step)},
+                    model_dir + 'checkpoint-%d.pt' % int(global_step))
 
     def load(self, model_dir, checkpoint=None):
         save_file, save_step = None, 0

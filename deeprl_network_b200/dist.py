@@ -75,6 +75,22 @@ def gather_to_root(obj):
     return parts
 
 
+def concat_envs(parts, axes):
+    """Per-env tensors of every rank ({name: tensor}, in rank order) -> the run's tensors in global env order, each
+    concatenated along its env axis axes[name]."""
+    return {k: torch.cat([p[k] for p in parts], dim=axes[k]) for k in parts[0]}
+
+
+def take_envs(tensors, axes, env0, n):
+    """The envs env0 .. env0 + n - 1 of per-env tensors in global env order ({name: tensor}, env axis axes[name])."""
+    out = {}
+    for k, t in tensors.items():
+        if env0 < 0 or env0 + n > t.shape[axes[k]]:
+            raise ValueError('%s holds %d envs, not the envs %d .. %d' % (k, t.shape[axes[k]], env0, env0 + n - 1))
+        out[k] = t.narrow(axes[k], env0, n)
+    return out
+
+
 def check_replicas(tensors):
     """Raise RuntimeError on every rank unless all ranks hold bit-identical copies of the tensors {name: tensor}
     (the data-parallel replicas of the weights and optimizer state)."""

@@ -25,6 +25,7 @@ import numpy as np
 import torch
 
 from .. import _lib as L
+from .. import dist as D
 
 
 def chain_masks(n):
@@ -272,6 +273,31 @@ class CACCEnv:
                                         L.ptr(self.hs), L.ptr(self.vs), L.ptr(self.us), L.ptr(self.t_dev),
                                         L.ptr(self.collision_dev), L.ptr(self.v_init), L.ptr(obs), obs.shape[-1],
                                         L.ptr(rew), L.ptr(grew), L.ptr(done), L.stream()), 'nmarl_cacc_step')
+
+    # per-env device state kept in a snapshot, and the env axis of each ([agent][env] arrays: 1; [env] arrays: 0).
+    # Not kept: _action_dev and _u01 (staging of the one-env host API, written before they are read) and _mask0
+    # (a constant).
+    SNAPSHOT_AXES = dict(hs=1, vs=1, us=1, v_init=1, t_dev=0, collision_dev=0, episode_dev=0, obs_dev=1, fp_dev=1,
+                         reward_dev=1, greward_dev=0, done_dev=0, env_par=0)
+
+    def snapshot(self):
+        """Host copy of every per-env device tensor: vehicle state, leader profile (v_init), step and episode counters,
+        collision / done latches, the per-env parameter table and the env's own observation / reward buffers.
+        -> {'envs': {name: tensor}, 'env_axis': {name: env axis}}."""
+        envs = {k: getattr(self, k).cpu() for k in self.SNAPSHOT_AXES if getattr(self, k) is not None}
+        return dict(envs=envs, env_axis={k: self.SNAPSHOT_AXES[k] for k in envs})
+
+    def restore(self, snap):
+        """Copy a snapshot (global env order) into this env's tensors in place: the envs env0 .. env0 + n_env - 1."""
+        if ('env_par' in snap['envs']) != (self.env_par is not None):
+            raise ValueError('the snapshot %s per-env scenario parameters and this config %s' % (
+                'has' if 'env_par' in snap['envs'] else 'has no', 'has' if self.env_par is not None else 'has none'))
+        envs = D.take_envs(snap['envs'], snap['env_axis'], self.env0, self.n_env)
+        for k, v in envs.items():
+            dst = getattr(self, k)
+            if tuple(v.shape) != tuple(dst.shape):
+                raise ValueError('snapshot tensor %s has shape %s, this env needs %s' % (k, tuple(v.shape), tuple(dst.shape)))
+            dst.copy_(v)
 
     @property
     def cfg_seed(self):

@@ -371,6 +371,33 @@ class VecTrainer:
             summary_writer.add_scalar('train_reward', mean, int(global_step))
         return mean
 
+    def snapshot(self):
+        """The run state between two updates, in a layout that depends neither on the process count nor on the kernel
+        path: the engine's and the env's (per-env tensors in global env order, gathered from every rank), the update
+        count, the env reset seed, the schedule position and the records behind train_reward.csv / env_par.csv.  Every
+        rank calls it (it checks that the Philox state agrees and gathers); rank 0 gets the snapshot, the others None."""
+        D.check_replicas({'Philox state (engine.rng)': self.engine.rng})
+        eng, env = self.engine.snapshot(), self.env.snapshot()
+        parts = D.gather_to_root((eng['envs'], env['envs']))
+        if parts is None:
+            return None
+        eng['envs'] = D.concat_envs([p[0] for p in parts], eng['env_axis'])
+        env['envs'] = D.concat_envs([p[1] for p in parts], env['env_axis'])
+        return dict(engine=eng, env=env, n_update=self.n_update, seed=int(self._seed),
+                    schedule_n=self.model.lr_scheduler.n,data=plain_records(self.data),
+                    par_data=plain_records(self.par_data))
+
+    def restore(self, snap):
+        """Put a snapshot back in place: after start() and before the first update, so that the CUDA graph the first
+        update captures reads the restored tensors.  Each rank takes its own envs of the snapshot's global order."""
+        if self.graph is not None or self.n_update:
+            raise RuntimeError('VecTrainer.restore runs after start() and before the first update')
+        self.engine.restore(snap['engine'])
+        self.env.restore(snap['env'])
+        self.n_update, self._seed = int(snap['n_update']), int(snap['seed'])
+        self.model.lr_scheduler.n = snap['schedule_n']
+        self.data, self.par_data = list(snap['data']), list(snap['par_data'])
+
     def write_csv(self, output_path):
         """train_reward.csv and, with per-env scenario parameters, env_par.csv: per log record the mean / min / max over
         the batch of every drawn field (the table as it stands at the record: the parameters of the running episodes)."""
@@ -539,6 +566,19 @@ class BatchedEvaluator:
     def write_csv(self, output_path):
         import pandas as pd
         pd.DataFrame(self.data).to_csv(output_path + 'test_reward.csv')
+
+    def snapshot(self):
+        """The test_reward.csv records so far (a resumed run writes the file whole)."""
+        return plain_records(self.data)
+
+    def restore(self, records):
+        self.data = list(records)
+
+
+def plain_records(records):
+    """Records with NumPy scalars turned into Python numbers, which a snapshot loads without unpickling code (and
+    which pandas writes to CSV exactly like the NumPy scalars)."""
+    return [{k: v.item() if isinstance(v, np.generic) else v for k, v in r.items()} for r in records]
 
 
 def split_episodes(first, steps, action, reward, hs, vs, us):

@@ -20,6 +20,18 @@ and the gradient is summed over the ranks, which gives the training run of one p
 order of floating-point sums.  Rank 0 alone writes the log, the files under data/ and the checkpoint.  NCCL when every
 rank has a GPU of its own, else gloo (ranks sharing a GPU; no CUDA graphs).  Refused with a ValueError: n_env not
 divisible by the process count, n_env = 1, and evaluate under torchrun (INTEGRATION §4).
+
+With n_env > 1 a run can survive its process.  TRAIN_CONFIG.checkpoint_interval (environment steps) makes rank 0 write
+model/checkpoint-<step>.pt and the snapshot model/resume-<step>.pt at the first update boundary after each multiple
+(the newest 5 of each are kept), and
+
+    python main.py --base-dir D train --config-dir F.ini --resume
+
+continues from the newest D/model/resume-*.pt, also under torchrun with another process count.  F.ini must equal the
+snapshot's configuration except for a raised TRAIN_CONFIG.total_step; with lr_decay = linear the schedule's horizon is
+the new total_step from the resume point on, so the rate jumps there to lr_init (1 - n / new total_step) and ramps down
+to lr_min at the new end.  Refused with a ValueError on every rank: no snapshot, n_env = 1, an
+n_env other than the snapshot's, and any other configuration difference (INTEGRATION §4, DESIGN §5.1).
 """
 import argparse
 import configparser
@@ -29,6 +41,7 @@ import os
 from deeprl_network_b200.agents import models as agent_models
 from deeprl_network_b200.envs.cacc_env import CACCEnv, nominal_config
 from deeprl_network_b200 import dist as D
+from deeprl_network_b200 import resume as R
 from deeprl_network_b200 import utils as U
 
 AGENTS = {'ia2c': agent_models.IA2C, 'ia2c_fp': agent_models.IA2C_FP, 'ma2c_cu': agent_models.IA2C_CU,
@@ -42,6 +55,8 @@ def parse_args(argv=None):
     modes = top.add_subparsers(dest='option', help='train or evaluate')
     tr = modes.add_parser('train', help='train the agent named in the config under the base dir')
     tr.add_argument('--config-dir', type=str, default='./config/config_ma2c_nc_catchup.ini', help='experiment config path')
+    tr.add_argument('--resume', action='store_true',
+                    help='continue from the newest snapshot <base-dir>/model/resume-<step>.pt (n_env > 1)')
     ev = modes.add_parser('evaluate', help='evaluate the agent stored under the base dir')
     ev.add_argument('--evaluation-seeds', type=str, default=DEFAULT_EVAL_SEEDS, help='random seeds for evaluation, split by ,')
     ev.add_argument('--demo', action='store_true', help='accepted for compatibility (SUMO gui in the reference); no files are written')
@@ -82,29 +97,49 @@ def init_agent(env, config, total_step, seed, **kw):
                              total_step, config, seed=seed, n_env=env.n_env, **kw)
 
 
-def _train_batched(env, model, total_step, log_interval, writer=None, output_path=None, tester=None, graph=True):
+def _train_batched(env, model, total_step, log_interval, writer=None, output_path=None, tester=None, graph=True,
+                   resume=None, checkpoint_interval=0, checkpoint=None):
     """n_env > 1: whole updates on the device until total_step environment steps (summed over all envs of all
     processes) are done.
     Every `log_interval` environment steps one record goes to data/train_reward.csv (and the TB scalar
     `train_reward`): mean / std of the per-step global TRAINING reward of the last batch.  With a `tester`
     (BatchedEvaluator, TRAIN_CONFIG.greedy_test) each record also runs one greedy episode per ENV_CONFIG test seed
     with the current weights and adds a record to data/test_reward.csv (and the TB scalar `test_reward`).  In a run over
-    several processes every rank calls it; the records are taken on rank 0 (the others pass output_path None)."""
+    several processes every rank calls it; the records are taken on rank 0 (the others pass output_path None).
+    resume: a snapshot's run state, put in place before the first update.  With a checkpoint_interval (environment
+    steps), checkpoint(run state or None, env steps) is called at the first update boundary after each multiple."""
     loop = U.VecTrainer(env, model, graph=graph)
     loop.start()
-    done_steps, per_update = 0, model.n_step * env.n_env_total
+    if resume is not None:
+        loop.restore(resume['loop'])
+        if tester is not None:
+            tester.restore(resume['test'])
+    per_update = model.n_step * env.n_env_total
+    done_steps = loop.n_update * per_update
     every = max(1, int(log_interval) // per_update)
+
+    def log():
+        r = loop.log_rewards(done_steps, writer)
+        if r is not None:
+            logging.info('update %d, env steps %d, mean step reward %.2f' % (loop.n_update, done_steps, r))
+        if tester is not None:
+            r = tester.log_test(done_steps, env.test_seeds, writer)
+            if r is not None:
+                logging.info('update %d, env steps %d, greedy test reward %.2f' % (loop.n_update, done_steps, r))
     while done_steps < total_step:
         loop.update()
         done_steps += per_update
-        if loop.n_update % every == 0 or done_steps >= total_step:
-            r = loop.log_rewards(done_steps, writer)
-            if r is not None:
-                logging.info('update %d, env steps %d, mean step reward %.2f' % (loop.n_update, done_steps, r))
-            if tester is not None:
-                r = tester.log_test(done_steps, env.test_seeds, writer)
-                if r is not None:
-                    logging.info('update %d, env steps %d, greedy test reward %.2f' % (loop.n_update, done_steps, r))
+        on_cadence = loop.n_update % every == 0
+        if on_cadence:
+            log()
+        if checkpoint_interval and done_steps // checkpoint_interval > (done_steps - per_update) // checkpoint_interval:
+            run = loop.snapshot()                  # every rank takes part; rank 0 gets the run state
+            if run is not None:
+                checkpoint(dict(loop=run, test=None if tester is None else tester.snapshot()), done_steps)
+        if not on_cadence and done_steps >= total_step:
+            # the last update's record, off the cadence: taken after the snapshot, so that a run resumed from it (and
+            # trained longer) writes the records of the uninterrupted run
+            log()
     if output_path is not None:
         loop.write_csv(output_path)
         if tester is not None:
@@ -113,21 +148,60 @@ def _train_batched(env, model, total_step, log_interval, writer=None, output_pat
     return done_steps
 
 
+def _resume_state(args, config_text, n_env):
+    """--resume: the newest snapshot under <base>/model/ after every check; raises ValueError (on every rank, before
+    any collective call) when there is none or it does not belong to this configuration."""
+    path = R.newest_snapshot(os.path.join(args.base_dir, 'model'))
+    if path is None:
+        raise ValueError('--resume: no snapshot resume-<step>.pt under %s' % os.path.join(args.base_dir, 'model'))
+    snap = R.load_snapshot(path)
+    R.check_resumable(snap, config_text, n_env)
+    return path, snap
+
+
+def _keep_one_ini(data_dir, name, config_text):
+    """A resumed run: data/<name> holds the configuration text it runs (written under a temporary name and renamed, so
+    that resuming from the .ini stored in data/ itself is safe), and every other .ini under data/ goes, so that
+    evaluate finds this one."""
+    tmp = os.path.join(data_dir, '.%s.%d.tmp' % (name, os.getpid()))
+    with open(tmp, 'w') as f:
+        f.write(config_text)
+    os.replace(tmp, os.path.join(data_dir, name))
+    for f in os.listdir(data_dir):
+        if f.endswith('.ini') and f != name:
+            os.remove(os.path.join(data_dir, f))
+
+
 def train(args):
     world, rank, _ = D.launch_world()
-    shard = backend = None
+    cfg = read_config(args.config_dir)
+    with open(args.config_dir) as f:
+        config_text = f.read()
+    n_env = cfg.getint('ENV_CONFIG', 'n_env', fallback=1)
+    interval = int(cfg.getfloat('TRAIN_CONFIG', 'checkpoint_interval', fallback=0))
+    resume = args.resume
+    shard = backend = snap = None
+    # refused on every rank before the process group exists
     if world > 1:
-        # refused on every rank before the process group exists
-        shard = D.env_shard(read_config(args.config_dir).getint('ENV_CONFIG', 'n_env', fallback=1), world, rank)
+        shard = D.env_shard(n_env, world, rank)
+    if (resume or interval) and n_env == 1:
+        raise ValueError('--resume and TRAIN_CONFIG.checkpoint_interval need batched training (ENV_CONFIG.n_env > 1); '
+                         'the one-env Trainer cannot be resumed')
+    if resume:
+        snap_path, snap = _resume_state(args, config_text, n_env)
+    if world > 1:
         backend = D.init_from_env()
     lead = rank == 0                                       # rank 0 alone writes the log, data/ and the checkpoint
     if lead:
         dirs = U.init_dir(args.base_dir)
         U.init_log(dirs['log'])
-        U.copy_file(args.config_dir, dirs['data'])         # evaluate finds the config next to the results
+        if resume:
+            _keep_one_ini(dirs['data'], os.path.basename(args.config_dir), config_text)
+            logging.info('Training: resume from %s at env step %d' % (snap_path, snap['step']))
+        else:
+            U.copy_file(args.config_dir, dirs['data'])     # evaluate finds the config next to the results
     else:
         logging.basicConfig(format='%(asctime)s [rank ' + str(rank) + '] %(message)s', level=logging.WARNING)
-    cfg = read_config(args.config_dir)
     steps = {k: int(cfg.getfloat('TRAIN_CONFIG', k)) for k in ('total_step', 'test_interval', 'log_interval')}
     env = init_env(cfg['ENV_CONFIG'], shard=shard)
     logging.info('Training: a dim %r, agent dim: %d' % (env.n_a_ls, env.n_agent))
@@ -143,9 +217,17 @@ def train(args):
     if shard is not None or env.n_env > 1:
         greedy_test = cfg.getboolean('TRAIN_CONFIG', 'greedy_test', fallback=False)
         tester = U.BatchedEvaluator(cfg['ENV_CONFIG'], model, world=world, rank=rank) if greedy_test else None
+
+        def checkpoint(run, step):                          # rank 0: the two files of a periodic checkpoint
+            model.save(dirs['model'], step)
+            R.save_snapshot(dirs['model'], step, run, config_text, env.n_env_total)
+            R.prune(dirs['model'])
+            logging.info('Training: checkpoint and snapshot at env step %d' % step)
         final_step = _train_batched(env, model, steps['total_step'], steps['log_interval'],
                                     U.make_summary_writer(dirs['log']) if lead else None,
-                                    dirs['data'] if lead else None, tester, graph=backend != 'gloo')
+                                    dirs['data'] if lead else None, tester, graph=backend != 'gloo',
+                                    resume=None if snap is None else snap['run'], checkpoint_interval=interval,
+                                    checkpoint=checkpoint)
     else:
         counter = U.Counter(steps['total_step'], steps['test_interval'], steps['log_interval'])
         U.Trainer(env, model, counter, U.make_summary_writer(dirs['log']), output_path=dirs['data']).run()
@@ -156,6 +238,8 @@ def train(args):
     if lead:
         logging.info('Training: save final model at step %d ...' % final_step)
         model.save(dirs['model'], final_step)
+        if interval:
+            R.prune(dirs['model'])
     D.shutdown()
 
 
